@@ -64,7 +64,28 @@ def parse_args():
                     help="reference arm: wall-clock budget for all steps; the per-step sample shrinks to fit")
     ap.add_argument("--lanes", type=int, default=6, help="tracks in flight per GPU for the device-resident number")
     ap.add_argument("--opt", action="append", default=[], help="library switch name=value (A/B measurements)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed device-resident path returned in its last step as DIR/<name>.npy "
+                         f"(float32; a fixed, seeded sample of rows when the whole would exceed {MAX_DUMP_BYTES // 10**6} MB)")
     return ap.parse_args()
+
+
+MAX_DUMP_BYTES = 64_000_000
+DUMP_SAMPLE_ROWS = 1 << 21
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Each (frames, 2) array whole, or, when all of them would not fit MAX_DUMP_BYTES, the same seeded,
+    sorted sample of DUMP_SAMPLE_ROWS rows of each plus the row numbers as `<name>_rows.npy` (float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > MAX_DUMP_BYTES and len(a) > DUMP_SAMPLE_ROWS:
+            rows = np.sort(np.random.default_rng(0).choice(len(a), DUMP_SAMPLE_ROWS, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def workload_config(args) -> dict:
@@ -74,7 +95,7 @@ def workload_config(args) -> dict:
     n = int(w["sample_rate"] * seconds)
     return {"workload": w["text"] if not args.seconds else w["text"] + f" [track length overridden: {seconds:.0f} s]",
             "name": args.workload, "sample_rate": w["sample_rate"], "frames_per_track": n,
-            "l2": "inputs larger than the 126 MB L2 between timed iterations: "
+            "l2": "inputs larger than the H100's 50 MB L2 between timed iterations: "
                   + ("3 rotating tracks per GPU, ~290 MB touched per step" if args.workload == "c2"
                      else f"one track is {n * 8 / 1e6:.0f} MB per signal"),
             "precision": "GPU arm: float32 I/O and FFTs, float64 reductions / FIR design / IIR state; CPU arm: float64"}
@@ -412,7 +433,7 @@ def run_b200(args) -> dict:
         barrier()
         return ms
 
-    # ---- inputs: distinct tracks per rank, rotated, so no step finds its inputs in the 126 MB L2 (config 2:
+    # ---- inputs: distinct tracks per rank, rotated, so no step finds its inputs in the 50 MB L2 (config 2:
     # three 64 MB tracks; configs 3 and 5: one buffer of 0.46 / 1.27 GB, several times the L2 by itself)
     n_sets = 3 if name == "c2" else 1
     host_t, host_r, dev_t, dev_r = [], [], [], []
@@ -560,9 +581,12 @@ def run_b200(args) -> dict:
     sampler.begin()
     if is_limiter:
         dev_ms, launches = timed_events(step_device, args.steps, warm)
+        last_out = lim_out.cpu().numpy() if args.dump_outputs else None
         dev_serial_ms = dev_ms
     else:
         dev_ms, launches = timed_lanes(args.steps, warm)
+        # (copied now: lane 0 is reused by the passes below)
+        last_out = lane_out[(args.steps - 1) % n_lanes].cpu().numpy() if args.dump_outputs else None
         dev_serial_ms, _ = timed_events(step_device, args.steps, warm)
     seam_ms = timed_wall(step_seam, args.steps, warm)
     if pipe is not None:
@@ -573,8 +597,7 @@ def run_b200(args) -> dict:
     clocks = sampler.stop() if rank == 0 else None
     files_ms = None
     if files_dir is not None:  # outside the clock window: dominated by host file I/O
-        files_steps = min(args.steps, 5)
-        files_ms = timed_wall(step_files, files_steps, 2) / files_steps
+        files_ms = timed_wall(step_files, args.steps, 2) / args.steps
     if pipe is not None:
         pipe.close()
 
@@ -612,15 +635,10 @@ def run_b200(args) -> dict:
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet (not measured)"
         bpf = ALGORITHMIC_BYTES_PER_FRAME.get(dominant)
-        traffic_path = os.path.join(ROOT, "profiles", "traffic.json")
-        traffic = None
-        if os.path.exists(traffic_path):
-            table = json.load(open(traffic_path))
-            traffic = table.get(name, {}).get(dominant) if isinstance(table.get(name), dict) else (table.get(dominant) if name == "c2" else None)
         roofline = {"kernel": dominant, "bound": "hbm", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None,
-                    "traffic": traffic, "peak_source": peak_src, "avg_launch_ms": summary[dominant]["avg_ms"],
+                    "peak_source": peak_src, "avg_launch_ms": summary[dominant]["avg_ms"],
                     "algorithmic_bytes_per_launch": None}
         if bpf:
             alg = bpf * n
@@ -636,7 +654,8 @@ def run_b200(args) -> dict:
             # the FFT kernels sit under the FP32 roof, not the HBM one (DESIGN.md section 4): reported next to the
             # HBM figure, not instead of it
             props = torch.cuda.get_device_properties(device)
-            peak_ops = props.multi_processor_count * 128 * 1.965e9  # lanes x max SM clock
+            sm_max_hz = ((clocks or {}).get("sm_max_mhz") or 1980.0) * 1e6  # (1980 MHz: the H100 SXM's maximum)
+            peak_ops = props.multi_processor_count * 128 * sm_max_hz  # lanes x max SM clock
             ops = fp32_ops * n
             roofline["cuda_core"] = {"ops_per_launch": ops, "peak_top_per_s": peak_ops / 1e12,
                                      "frac": ops / (summary[dominant]["avg_ms"] * 1e-3) / peak_ops,
@@ -704,6 +723,8 @@ def run_b200(args) -> dict:
             "e2e": e2e, "gpu_launches": int(launches),
             "roofline": roofline, "kernels": summary, "cpu_baseline": cpu_baseline, "clocks": clocks,
         }
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"limited": last_out})
     if files_dir is not None:
         import shutil
         shutil.rmtree(files_dir, ignore_errors=True)
@@ -719,6 +740,8 @@ SHARED_SOCKET_MODE = "cached"
 
 def main():
     args = parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        raise SystemExit("--dump-outputs writes the CUDA path's outputs: it needs --impl b200")
     out = run_reference(args) if args.impl == "reference" else run_b200(args)
     if out:
         print(json.dumps(out))

@@ -1,4 +1,4 @@
-/* matchering_b200 -- C ABI of the B200-native Matchering hot path.
+/* matchering_b200 -- C ABI of the CUDA-native (H100, sm_90a) Matchering hot path.
  *
  * The reference (sergree/matchering v2.0.6) is pure Python and has no FFI layer; the seam this
  * library plugs into is the pair of Python call sites

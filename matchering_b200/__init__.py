@@ -1,4 +1,4 @@
-"""matchering_b200 -- B200-native drop-in for Matchering's mastering DSP hot path.
+"""matchering_b200 -- CUDA-native (H100, sm_90a) drop-in for Matchering's mastering DSP hot path.
 
 Public surface mirrors the reference package (matchering/__init__.py:31-36):
     mg.log, mg.Result, mg.pcm16, mg.pcm24, mg.Config, mg.process, mg.load, mg.check

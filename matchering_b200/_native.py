@@ -223,7 +223,7 @@ def load() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -m matchering_b200.build` "
-                "(nvcc, sm_100a). matchering_b200 has no CPU fallback.")
+                "(nvcc, sm_90a). matchering_b200 has no CPU fallback.")
         _LIB = bind(C.CDLL(LIB_PATH))
         if _LIB.mgb_version() < 200:
             raise ImportError("libmatchering_b200.so is older than this package")

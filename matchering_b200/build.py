@@ -1,4 +1,4 @@
-"""Build libmatchering_b200.so in-tree with nvcc for sm_100a (no torch extension machinery: the
+"""Build libmatchering_b200.so in-tree with nvcc for sm_90a, the H100 (no torch extension machinery: the
 library has a plain C ABI and is loaded with ctypes).  `python -m matchering_b200.build`."""
 from __future__ import annotations
 
@@ -15,8 +15,9 @@ LIB_PATH = os.path.join(PKG_DIR, "libmatchering_b200.so")
 SOURCES = ["api.cu", "analyze.cu", "design.cu", "convolve.cu", "correct.cu", "limiter.cu", "pipeline.cu", "hostio.cu", "resample.cu"]
 HEADERS = sorted(f for f in os.listdir(SRC_DIR) if f.endswith(".cuh")) + [os.path.join("..", "..", "include", "matchering_b200.h")]
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *GENCODE,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
@@ -66,7 +67,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         list(ex.map(run, jobs))
     if jobs or force or _stale(LIB_PATH, objs):
         # (--no-undefined: a symbol that only exists inside another file's anonymous namespace must fail here, not at dlopen)
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xlinker", "--no-undefined", "-o", LIB_PATH, *objs]
+        cmd = [nvcc, "-shared", *GENCODE, "-Xlinker", "--no-undefined", "-o", LIB_PATH, *objs]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

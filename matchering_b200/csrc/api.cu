@@ -72,7 +72,7 @@ int num_sms() {
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
             cached = n;
         else
-            cached = 148;
+            cached = 132;  // the H100 SXM's SM count
     }
     return cached;
 }

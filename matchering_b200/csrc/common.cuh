@@ -1,4 +1,4 @@
-// Shared device helpers for the matchering_b200 kernels (sm_100a).
+// Shared device helpers for the matchering_b200 kernels (sm_90a).
 //
 // The same sources are also compiled for the host by the test-only emulator
 // (tests/emul/cuda_emul.h, -DMGB_EMULATE); everything PTX-specific therefore lives behind the

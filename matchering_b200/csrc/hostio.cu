@@ -163,8 +163,8 @@ inline void widen_plain(const float* __restrict__ src, double* __restrict__ dst,
 // Streaming variants.  The staging chunk is written once by a worker and read once by the DMA engine, the result
 // array is written once and read by nobody here: a non-temporal store skips the read-for-ownership of every
 // destination line and -- what matters more for the ring -- leaves the line in memory instead of dirty in the
-// writing core's cache, where the DMA engine's reads would have to fetch it from (measured on the B200 host:
-// the ring drained at 13 GB/s from the cores' caches, at link speed from memory).  dst is 64-byte aligned by
+// writing core's cache, where the DMA engine's reads would have to fetch it from (a ring drained from the
+// cores' caches runs well below link speed; from memory it runs at link speed).  dst is 64-byte aligned by
 // construction for the ring (slices start on 16-sample boundaries of a pinned allocation).
 // MGB_HOST_NT: 0 = plain stores, 1 = 256-bit streaming stores, 2 = 512-bit where the CPU has them (default).
 // MGB_HOST_PREFETCH: software prefetch distance in bytes (0 = none).
@@ -416,9 +416,8 @@ int download(mgb_host_io* io, const float* d_src, void* h_dst, int dst_width, in
     MGB_REQUIRE(dst_width == 4 || dst_width == 8, MGB_ERR_INVALID, "host array must be float32 or float64");
     if (samples == 0) return MGB_OK;
     // float64 results into pinned memory, two routes.  (a) Widened on the device and copied by ONE DMA: twice the
-    // bytes over the link (2.4 ms for a 3-minute track at 54 GB/s), no host thread involved.  (b) Float32 chunks
-    // through the ring, widened by the workers with streaming stores: 1.7 ms for that track (tools/seam_ab.py,
-    // profiles/r02_seam_ab2.txt: 4.90 against 5.74 ms per stages.main call) -- but 50 % SLOWER than (a) on the
+    // bytes over the link, no host thread involved.  (b) Float32 chunks through the ring, widened by the workers
+    // with streaming stores: faster for a 3-minute track (tools/seam_ab.py compares the two), slower than (a) on the
     // one-hour limiter buffer (2.5 GB: the widening competes with itself for the socket's memory bandwidth).
     // So (b) up to 256 MB of float32 and (a) beyond; option host_download_ring = 0 / 2 forces (a) / (b).
     const bool prefer_ring = mgb_host_download_through_ring(samples) != 0;
@@ -533,10 +532,9 @@ extern "C" {
 int mgb_host_io_create(int32_t threads, int64_t chunk_samples, int32_t ring, mgb_host_io** out) {
     MGB_REQUIRE(out != nullptr, MGB_ERR_INVALID, "host_io: NULL argument");
     if (threads <= 0) {
-        // The conversion is what bounds a transfer (each worker narrows 7-8 GB/s of float64 source on the B200
-        // host, the link takes 108 GB/s of it), so every core helps -- up to what the process may use: the
-        // affinity mask, and the cgroup's CPU quota (the B200 boxes grant 16 cores per GPU; workers that spin
-        // past the quota get the whole process throttled).  Three cores stay free for the issuing thread, the
+        // The conversion is what bounds a transfer (one worker narrows float64 source far slower than the link
+        // takes it), so every core helps -- up to what the process may use: the affinity mask, and the cgroup's
+        // CPU quota (workers that spin past the quota get the whole process throttled).  Three cores stay free for the issuing thread, the
         // driver's threads and the caller's own.
         int usable = (int)std::thread::hardware_concurrency();
 #if defined(__linux__)
@@ -560,16 +558,13 @@ int mgb_host_io_create(int32_t threads, int64_t chunk_samples, int32_t ring, mgb
 #endif
         threads = usable >= 19 ? 16 : (usable > 4 ? usable - 3 : (usable > 1 ? usable - 1 : 1));
     }
-    // A ring of six 4 MB chunks, written with streaming stores.  Measured on the B200 host (Xeon 8562Y+, 16 cores
-    // of quota per GPU), one process (tools/seam_ab.py, alternating calls; profiles/r02_seam_ab.txt, r02_seam_ab2.txt):
-    // with ordinary stores the DMA engine has to pull every line out of the writing core's cache and the ring
-    // drains at 13 GB/s, whatever its size (6.9-7.0 ms per stages.main call; demoting the lines to the last-level
-    // cache with CLDEMOTE after writing them: 5.9-6.9 ms); with streaming stores the chunks sit in memory and the
-    // ring drains at link speed (5.7 ms; 4.9 ms with the result coming back through the ring as well).  Larger chunks
-    // mean fewer copies, and a download pays ~18 us per copy: 2 MB chunks 5.20 ms, 4 MB 4.90, 8 MB 5.01.
+    // A ring of six 4 MB chunks, written with streaming stores (tools/seam_ab.py and tools/seam_sweep.py compare
+    // geometries): with ordinary stores the DMA engine has to pull every line out of the writing core's cache and
+    // the ring drains well below link speed, whatever its size; with streaming stores the chunks sit in memory and
+    // the ring drains at link speed.  Larger chunks mean fewer copies, and a download pays a fixed cost per copy.
     // With ordinary stores (MGB_HOST_NT=0) the best geometry is sixteen 256 KB chunks, which stay in the
     // cores' caches: that is what several processes sharing one socket's memory bandwidth should use
-    // (tools/gpu_n4_sweep.sh: 7.8 ms per call against 14.3 ms with twelve 1 MB chunks going through memory).
+    // (tools/gpu_n4_sweep.sh compares the two with four processes on one socket).
     if (chunk_samples <= 0) chunk_samples = g_stream_stores ? 1 << 20 : 1 << 16;
     if (ring <= 0) ring = g_stream_stores ? 6 : 16;
     MGB_REQUIRE(threads <= 256 && ring <= 64 && chunk_samples % 16 == 0, MGB_ERR_INVALID, "host_io: bad geometry");

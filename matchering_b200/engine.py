@@ -1,5 +1,5 @@
 """Device-side session objects: PyTorch is the memory manager and stream provider, the compute
-is libmatchering_b200 (hand-written sm_100a kernels behind the C ABI).
+is libmatchering_b200 (hand-written sm_90a kernels behind the C ABI).
 
 DevicePlan   Config-only tables on one GPU (cached per device + Config).
 TrackSession the buffers of one mastering job of fixed sizes; calls the four stage entry points
@@ -20,7 +20,7 @@ _PLAN_CACHE: dict = {}
 
 def _require_cuda() -> None:
     if not torch.cuda.is_available():
-        raise RuntimeError("matchering_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("matchering_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
 
 
 def _stream_ptr(device) -> C.c_void_p:

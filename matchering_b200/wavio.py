@@ -93,8 +93,8 @@ _IO_SLICE = 4 << 20
 
 def _sliced_io(fd: int, view: memoryview, offset: int, write: bool) -> None:
     """pread / pwrite of a large buffer in 4 MB slices on a few threads (the calls release the GIL): the copy between
-    the page cache and the (pinned) buffer is a single-threaded memcpy per call, 5 GB/s; eight of them in parallel read
-    a 32 MB track in 1.5 ms instead of 6.5 (measured on the B200 host; writes of new files did not gain)."""
+    the page cache and the (pinned) buffer is a single-threaded memcpy per call; eight of them in parallel read a
+    track several times faster (writes of new files did not gain)."""
     global _IO_POOL
     n = len(view)
     if n <= _IO_SLICE:

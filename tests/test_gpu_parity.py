@@ -1,4 +1,4 @@
-"""Parity of the CUDA path (libmatchering_b200.so on a real B200) against the oracle and the
+"""Parity of the CUDA path (libmatchering_b200.so on a real H100) against the oracle and the
 golden vectors.  Everything goes through the C ABI, either directly or through the reference-shaped
 Python surface (stages.main / limiter.limit).  Tolerance: sample-wise max-abs <= 1e-5 (north star);
 the float64 FIR design is held to 1e-9."""
@@ -600,7 +600,7 @@ def test_kernel_variants_behind_switches_agree(torch_cuda, lib):
     import port
     from matchering_b200 import stages
     cfg = _config(max_piece_size=15.0)
-    n = 44100 * 120 + 77  # 431 frames of 12288 outputs on 148 SMs: two or three per CTA
+    n = 44100 * 120 + 77  # 431 frames of 12288 outputs on 132 SMs: three or four per CTA
     t, r = port.synth_target(n, 41), port.synth_reference(n - 4321, 42)
     want = port.main(t.astype(np.float64), r.astype(np.float64), cfg, True, True, True)
     got = {}

@@ -1,5 +1,5 @@
-"""oracle/port.py pinned: against the golden vectors generated from the unmodified reference
-(always), and against the reference itself where /root/reference exists."""
+"""oracle/port.py pinned against golden vectors generated from the unmodified reference
+(oracle/make_golden.py, oracle/make_golden_parity.py)."""
 import numpy as np
 import pytest
 
@@ -52,61 +52,54 @@ def test_limiter_early_out_returns_input_object():
     assert port.limit(x, port.OracleConfig()) is x
 
 
-# ---- against the live reference (build container only) -------------------------------------------
-def test_identities_against_reference_helpers(reference_package):
-    from matchering import Config, dsp
-    from matchering.limiter import hyrax
-    from matchering.stage_helpers import match_frequencies as mf
-    rng = np.random.default_rng(5)
-    g = np.abs(rng.standard_normal(5000)) * (rng.uniform(size=5000) > 0.7)
+# ---- against the unmodified reference's outputs for the same inputs (oracle/make_golden_parity.py) ---
+def test_identities_against_reference_helpers(golden, reference_surface):
+    from make_golden_parity import digest, identity_inputs
+    g_ref, want = golden("reference_parity.npz"), reference_surface["identity_digests"]
+    g, pieces, x = identity_inputs()
     for attack in (44, 45, 96):
-        want = getattr(hyrax, "__sliding_window_fast")(g, attack, "attack")
         reach = (attack + 1 if not attack & 1 else attack) - 1
-        assert np.array_equal(port.centred_max(g, reach), want)
+        assert digest(port.centred_max(g, reach)) == want[f"attack_window_{attack}"]
     for hold in (44, 45, 96, 3):
-        want = getattr(hyrax, "__sliding_window_fast")(g, hold, "hold")
-        assert np.array_equal(port.trailing_max(g, hold), want)
-    cfg = Config()
-    att, slided = getattr(hyrax, "__process_attack")(np.copy(g), cfg)
-    k = port.limiter_coefficients(port.config_from(cfg))
-    assert np.abs(port.one_pole_forward_backward(slided, k["c"]) - att).max() < 1e-15
-    pieces = rng.standard_normal((3, 20000))
-    want = getattr(mf, "__average_fft")(pieces, 44100, 4096)
+        assert digest(port.trailing_max(g, hold)) == want[f"hold_window_{hold}"]
+    k = port.limiter_coefficients(port.config_from(port.OracleConfig()))
+    att = port.one_pole_forward_backward(port.centred_max(g, k["reach"]), k["c"])
+    every = int(g_ref["attack_stride"])
+    assert np.abs(att[::every] - g_ref["process_attack_rows"]).max() < 1e-15
+    assert abs(att.sum() - float(g_ref["process_attack_sum"])) < 1e-12
     flat = pieces.reshape(-1)
     got = port.average_spectrum(flat, 20000, np.ones(3, dtype=bool), 4096)
-    assert np.abs(got - want).max() < 1e-15
-    x = rng.standard_normal((1000, 2))
-    mid, side = dsp.lr_to_ms(x)
+    assert np.abs(got - g_ref["average_fft"]).max() < 1e-15
     m2, s2 = port.mid_side(x)
-    assert np.array_equal(mid, m2) and np.array_equal(side, s2)
+    assert digest(m2) == want["mid"] and digest(s2) == want["side"]
 
 
 @pytest.mark.parametrize("sr,seconds", [(44100, 6.0), (96000, 2.5)])
-def test_main_against_reference(reference_package, sr, seconds):
-    from matchering import Config, stages
-    n = int(sr * seconds)
-    t = port.synth_target(n, 3).astype(np.float64)
-    r = port.synth_reference(n - 777, 4).astype(np.float64)
-    cfg = Config(internal_sample_rate=sr, max_piece_size=1.0)
-    want = stages.main(t, r, cfg, True, True, True)
+def test_main_against_reference(golden, sr, seconds):
+    from make_golden_parity import main_inputs
+    g = golden("reference_parity.npz")
+    every = int(g["main_stride"])
+    t, r = main_inputs(sr, seconds)
+    cfg = port.OracleConfig(internal_sample_rate=sr, max_piece_size=1.0)
     got = port.main(t, r, cfg, True, True, True)
-    for a, b in zip(got, want):
-        assert np.abs(a - b).max() < 1e-12
+    for name, a in zip(("limited", "no_limiter", "normalized"), got):
+        key = f"main_{sr}_{name}"
+        assert np.abs(a[::every] - g[key + "_rows"]).max() < 1e-12
+        # the whole array, through its sums: a difference anywhere of more than ~1e-12 per sample shows
+        assert np.abs(a.sum(axis=0) - g[key + "_sum"]).max() < 1e-12 * len(a)
+        assert np.abs((a * a).sum(axis=0) - g[key + "_sumsq"]).max() < 1e-12 * len(a)
 
 
 @pytest.mark.parametrize("n,whole", [(30000, False), (9000, True), (12000 + 4000 * 3, False)])
-def test_preview_pieces_against_reference(reference_package, monkeypatch, n, whole):
-    """oracle/port.py::preview_pieces against the unmodified create_preview (its two `save` calls captured)."""
-    from matchering import Config, Result, preview_creator
-    cfg = Config(internal_sample_rate=2000, preview_size=6, preview_analysis_step=2)
-    saved = {}
-    monkeypatch.setattr(preview_creator, "save", lambda file, arr, sr, subtype, name: saved.__setitem__(name, arr.copy()))
-    target = 2.5 * port.synth_target(n, 41).astype(np.float64)
-    result = port.synth_reference(n, 42).astype(np.float64) * (0.2 + np.abs(np.sin(np.linspace(0, 9, n))))[:, None]
-    keep_t, keep_r = target.copy(), result.copy()
-    preview_creator.create_preview(target, result, cfg, Result("t.wav", "PCM_16"), Result("r.wav", "PCM_16"))
-    index, t_piece, r_piece = port.preview_pieces(keep_t, keep_r, cfg)
-    assert np.array_equal(saved["target preview"], t_piece) and np.array_equal(saved["result preview"], r_piece)
+def test_preview_pieces_against_reference(reference_surface, n, whole):
+    """oracle/port.py::preview_pieces against the arrays the unmodified create_preview handed to its two
+    `save` calls, kept as digests of their bytes."""
+    import matchering_b200 as mg
+    from make_golden_parity import digest, preview_inputs
+    cfg = mg.Config(internal_sample_rate=2000, preview_size=6, preview_analysis_step=2)
+    index, t_piece, r_piece = port.preview_pieces(*preview_inputs(n), cfg)
+    want = reference_surface["preview_digests"][str(n)]
+    assert digest(t_piece) == want["target"] and digest(r_piece) == want["result"]
     assert (len(r_piece) == n) == whole
     if not whole:
         assert r_piece[0].tolist() == [0.0, 0.0] and r_piece[-1].tolist() == [0.0, 0.0]
