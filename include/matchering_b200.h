@@ -156,8 +156,7 @@ const char* mgb_last_error_string(void);
  * forward pass, the spectral product, the first inverse pass and the epilogue in registers (1, default,
  * fft_size 4096 and 8192) or sends every pass through shared memory (0).  "conv_frame": overlap-save
  * frame of the convolution in FIR lengths, 4 (default: a 4F-point transform pair yields 3F outputs; fft_size
- * 2048 and 4096 with pieces of at least 3F samples) or 2 (2F-point pair, F outputs).  "clip_ctas_per_sm": grid of
- * the RMS-correction passes in CTAs per SM (1..16, default 3).  "conv_persistent": the 16384-point convolution frames are
+ * 2048 and 4096 with pieces of at least 3F samples) or 2 (2F-point pair, F outputs).  "conv_persistent": the 16384-point convolution frames are
  * walked by one CTA per SM with the next frame's bulk copy under the epilogue (1, default) or take one CTA each (0).
  * "analyze_chain": the analysis FFT builds twiddle powers in registers (1, default) or reads them all (0).  "design_direct": mgb_test_design_fir runs the
  * spline/LOWESS chain directly even when the plan has a smoothing operator.  "lookback_inclusive":
@@ -204,8 +203,10 @@ int mgb_match_levels(const mgb_plan* plan, const mgb_track_layout* layout, const
  * FIR design for mid and side (match_frequencies.get_fir, :78-101, incl. __smooth_exponentially
  * :45-75 and dsp.smooth_lowess) and convolution of the level-matched target with both FIRs
  * (match_frequencies.convolve :104-119 == scipy fftconvolve 'same'), mid/side -> L/R
- * (dsp.ms_to_lr, dsp.py:67-68).  Writes the un-corrected result (d_result_lr), its mid channel
- * (workspace) and the first correction step's per-piece sum(clip(mid)^2).
+ * (dsp.ms_to_lr, dsp.py:67-68).  Writes the un-corrected result (d_result_lr), the first correction
+ * step's per-piece sum(clip(mid)^2) and, per piece, the list of mid samples loud enough that a later
+ * correction step may clip them (workspace).  The later stages read d_result_lr again: it must stay
+ * unchanged until mgb_finalize has run.
  * d_fir_out (optional, may be NULL): [2][F] doubles, the mid and side FIRs, for inspection. */
 int mgb_match_frequencies(const mgb_plan* plan, const mgb_track_layout* layout, const float* d_target_lr,
                           float* d_result_lr, double* d_fir_out, void* d_workspace, mgb_track_state* d_state,
@@ -213,7 +214,8 @@ int mgb_match_frequencies(const mgb_plan* plan, const mgb_track_layout* layout, 
 
 /* ---- stage 3: stages.__correct_levels (stages.py:138-170) -----------------------------------
  * rms_correction_steps iterations of clip -> per-piece RMS -> loudest mask -> coefficient.  The
- * coefficients accumulate in d_state->gain; the samples are scaled once, by the consumer. */
+ * coefficients accumulate in d_state->gain; the samples are scaled once, by the consumer.  A step
+ * reads the loud lists, or the result of mgb_match_frequencies where a list cannot give the exact sum. */
 int mgb_correct_levels(const mgb_plan* plan, const mgb_track_layout* layout, void* d_workspace,
                        mgb_track_state* d_state, void* stream);
 

@@ -17,7 +17,6 @@ int g_analyze_chain = 1;
 int g_conv_persistent = 1;
 int g_conv_fused = 1;
 int g_conv_ovs = 4;
-int g_clip_ctas_per_sm = 3;
 int g_lookback_inclusive = 1;
 int g_limiter_ticket = 0;
 
@@ -104,10 +103,13 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     w.design = (double*)take(8 * w.design_stride * 8);  // 2 channels x up to 4 design CTAs
     w.h_mid = (float2*)take((2 * F + 1) * 8);           // FIR spectrum bins 0..N/2 of the N = 2F or 4F grid
     w.h_side = (float2*)take((2 * F + 1) * 8);
-    w.mid_plane = (float*)take(L.target_frames * 4);
+    w.loud_capacity = loud_capacity(L.target_piece);
+    w.loud_values = (float*)take(w.loud_capacity * L.target_divisions * 4);
+    w.result_slot = (const float2**)take(8);
     w.conv_scratch = (float2*)take(conv_global_scratch_bytes(plan.fft_size, L.target_frames));
     w.zero_begin = base ? base + off : nullptr;
     w.piece_sums = (double*)take((int64_t)MGB_MAX_CORRECTION_STEPS * L.target_divisions * 8);
+    w.loud_count = (unsigned*)take((int64_t)L.target_divisions * 4);
     w.zero_end = base ? base + off : nullptr;
     // zeroed by mgb_finalize right before every limiter launch (a second finalize on the same track
     // must not find the first one's tickets and published carries)
@@ -285,11 +287,6 @@ int mgb_set_option(const char* name, int value) {
     MGB_REQUIRE(name != nullptr, MGB_ERR_INVALID, "option name is NULL");
     if (strcmp(name, "tma") == 0) {
         g_use_tma = value ? 1 : 0;
-        return MGB_OK;
-    }
-    if (strcmp(name, "clip_ctas_per_sm") == 0) {
-        MGB_REQUIRE(value >= 1 && value <= 16, MGB_ERR_INVALID, "clip_ctas_per_sm must be 1..16");
-        g_clip_ctas_per_sm = value;
         return MGB_OK;
     }
     if (strcmp(name, "conv_frame") == 0) {
@@ -514,11 +511,12 @@ int mgb_correct_levels(const mgb_plan* plan, const mgb_track_layout* L, void* d_
     MGB_TRY(check_aligned(d_workspace, "d_workspace"));
     cudaStream_t st = (cudaStream_t)stream;
     Workspace ws = carve_workspace(*plan, *L, d_workspace);
-    // step 0's per-piece sums come out of the convolution kernel's epilogue (gain is still 1 there);
-    // each later step is one pass over the mid plane that first derives the previous step's
-    // coefficient from that step's sums; a last small kernel closes the chain and writes the scalars
-    // __finalize needs.
-    for (int step = 1; step < plan->rms_correction_steps; ++step) MGB_TRY(launch_clip_sumsq(*plan, *L, ws, step, d_state, st));
+    // step 0's per-piece sums and loud lists come out of the convolution kernel's epilogue (gain is
+    // still 1 there); each later step is one pass over the loud lists (over the result, for a piece
+    // whose list overflowed or at a gain where quiet samples could clip: the result must be unchanged
+    // since mgb_match_frequencies) that first derives the previous step's coefficient from that step's
+    // sums; a last small kernel closes the chain and writes the scalars __finalize needs.
+    for (int step = 1; step < plan->rms_correction_steps; ++step) MGB_TRY(launch_loud_sumsq(*plan, *L, ws, step, d_state, st));
     return launch_correction_final(*plan, *L, ws, d_state, st);
 }
 

@@ -162,11 +162,12 @@ __device__ __forceinline__ void conv_apply_pair(cpx<float>& zk, cpx<float>& zn, 
 }
 
 // Output side of a frame of OUT outputs: circular index F-1+o of the inverse transform is output sample n0+o.
-// mid/side -> L/R (dsp.ms_to_lr), the first RMS-correction step's sum of clip(mid)^2 per piece, the peak.
+// mid/side -> L/R (dsp.ms_to_lr), the first RMS-correction step's sum of clip(mid)^2 per piece, the peak,
+// and the loud lists of the later correction steps (kernels.cuh: kLoudMid).
 template <int OUT>
 struct ConvEpilogue {
     float2* res;
-    float* midp;
+    LoudList loud;
     int valid, boundary, count_to;
     long long pa;
     int divisions;
@@ -174,10 +175,11 @@ struct ConvEpilogue {
     bool full;  // every output of the frame exists, is counted, belongs to piece pa, no channel is silent: nothing to test per sample
     double sq_a = 0.0, sq_b = 0.0;
     float peak = 0.0f;
-    __device__ __forceinline__ ConvEpilogue(float2* result, float* mid_plane, long long n0, long long frames,
+    __device__ __forceinline__ ConvEpilogue(float2* result, const LoudList& loud_, long long n0, long long frames,
                                             long long piece, int divisions_, const ConvBalance& bal) {
         res = result + n0;
-        midp = mid_plane + n0;
+        loud = loud_;
+        if (n0 == 0 && threadIdx.x == 0) *loud.result_slot = result;  // for the correction steps' full passes
         valid = (int)((frames - n0 < OUT) ? frames - n0 : OUT);
         const long long counted = piece * divisions_;  // samples that enter the piece RMS (dsp.unfold)
         pa = n0 / piece;
@@ -194,7 +196,6 @@ struct ConvEpilogue {
         const float m = y.x, sd = y.y;
         const float l = m + sd, r = m - sd;
         res[o] = make_float2(l, r);
-        midp[o] = m;
         peak = fmaxf(peak, fmaxf(fabsf(l), fabsf(r)));
         const float cf = fminf(1.0f, fmaxf(-1.0f, m));  // dsp.clip
         sq_a += (double)cf * (double)cf;
@@ -205,12 +206,54 @@ struct ConvEpilogue {
             const float m = mid_silent ? 0.0f : y.x, sd = side_silent ? 0.0f : y.y;
             const float l = m + sd, r = m - sd;
             res[o] = make_float2(l, r);
-            midp[o] = m;
             peak = fmaxf(peak, fmaxf(fabsf(l), fabsf(r)));
             if (o < count_to) {
                 const float cf = fminf(1.0f, fmaxf(-1.0f, m));  // dsp.clip
                 const double c2 = (double)cf * (double)cf;
                 if (o < boundary) sq_a += c2; else sq_b += c2;
+            }
+        }
+    }
+    // Appends the loud ones among K outputs per thread to the loud lists: outputs(k) is the k-th output's
+    // index o (< 0: none), mids(k) its transform value's real part.  Every lane of the warp calls, with
+    // the same K; per warp and piece one atomicAdd reserves the room for all K.  Entries past a list's
+    // capacity are dropped, but still counted: the correction steps see the overflow and do not use it.
+    template <int K, typename O, typename M>
+    __device__ __forceinline__ void append_loud(O outputs, M mids) {
+        const unsigned lane = threadIdx.x & 31u, below = (1u << lane) - 1u;
+        auto loud_in = [&](int k, bool second) {  // counted, loud, and in piece pa (second: pa + 1)
+            const int o = outputs(k);
+            if (o < 0 || o >= count_to || mid_silent) return false;
+            return fabsf(mids(k)) >= kLoudMid && (o >= boundary) == second;
+        };
+        unsigned na = 0, nb = 0;
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            na += __popc(__ballot_sync(0xffffffffu, loud_in(k, false)));
+            if (!full) nb += __popc(__ballot_sync(0xffffffffu, loud_in(k, true)));
+        }
+        unsigned base_a = 0, base_b = 0;
+        if (lane == 0) {
+            if (na) base_a = atomicAdd(&loud.count[pa], na);
+            if (nb) base_b = atomicAdd(&loud.count[pa + 1], nb);
+        }
+        if (na == 0 && nb == 0) return;
+        base_a = __shfl_sync(0xffffffffu, base_a, 0);
+        base_b = __shfl_sync(0xffffffffu, base_b, 0);
+        float* row_a = loud.values + pa * loud.capacity;
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            const bool a = loud_in(k, false);
+            const unsigned ba = __ballot_sync(0xffffffffu, a);
+            const unsigned ia = base_a + __popc(ba & below);
+            if (a && ia < loud.capacity) row_a[ia] = mids(k);
+            base_a += __popc(ba);
+            if (!full) {
+                const bool b = loud_in(k, true);
+                const unsigned bb = __ballot_sync(0xffffffffu, b);
+                const unsigned ib = base_b + __popc(bb & below);
+                if (b && ib < loud.capacity) row_a[loud.capacity + ib] = mids(k);
+                base_b += __popc(bb);
             }
         }
     }
@@ -267,7 +310,7 @@ template <int F, bool CHAIN>
 __global__ void __launch_bounds__(F / 8, (F <= 4096 ? 2 : 1))
 convolve_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                 const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
-                const float2* __restrict__ h_side, float2* __restrict__ result, float* __restrict__ mid_plane,
+                const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
                 double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, int use_tma) {
     constexpr int N = 2 * F;
     constexpr int THREADS = N / 16;
@@ -303,12 +346,14 @@ convolve_kernel(const float2* __restrict__ x, long long frames, long long piece,
     __syncthreads();
 
     // ---- epilogue: coalesced stores -------------------------------------------------------------------
-    ConvEpilogue<F> ep(result, mid_plane, n0, frames, piece, divisions, bal);
+    ConvEpilogue<F> ep(result, loud, n0, frames, piece, divisions, bal);
 #pragma unroll
     for (int k = 0; k < F / THREADS; ++k) {
         const int o = tid + k * THREADS;
         if (o < ep.valid) ep.emit(o, planes.load(F - 1 + o));
     }
+    ep.template append_loud<F / THREADS>([&](int k) { return tid + k * THREADS; },
+                                         [&](int k) { return planes.load(F - 1 + tid + k * THREADS).x; });
     ep.finish(sp.red_a, sp.red_b, sp.red_f, piece_sums, state);
 }
 
@@ -334,7 +379,7 @@ template <int F, int OVS, bool CHAIN, bool PERSIST>
 __global__ void __launch_bounds__(OVS * F / 16, (OVS * F <= 8192 ? 2 : 1))
 convolve_fused_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                       const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
-                      const float2* __restrict__ h_side, float2* __restrict__ result, float* __restrict__ mid_plane,
+                      const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
                       double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, int use_tma, int nframes) {
     constexpr int N = OVS * F;
     constexpr int OUT = N - F;  // outputs per frame
@@ -413,7 +458,7 @@ convolve_fused_kernel(const float2* __restrict__ x, long long frames, long long 
         fft_middle<N, -1, THREADS, float, CHAIN, Inv>(planes, tw_inv);
 
         // ---- last inverse pass straight into the epilogue ------------------------------------------------
-        ConvEpilogue<OUT> ep(result, mid_plane, n0, frames, piece, divisions, bal);
+        ConvEpilogue<OUT> ep(result, loud, n0, frames, piece, divisions, bal);
         const cpx<float>* tw_last = tw_inv + fft_last_pass_twiddles<Inv>();
     #pragma unroll
         for (int p = 0; p < 2; ++p) {
@@ -441,6 +486,9 @@ convolve_fused_kernel(const float2* __restrict__ x, long long frames, long long 
                 for (int q = Q0; q < 8; ++q) ep.emit(j + 1 + (q - Q0) * NB8, v[q]);  // (o = OUT for j = NB8-1, q = 7: not valid)
                 if (j == NB8 - 1) ep.emit(0, v[Q0 - 1]);
             }
+            ep.template append_loud<8>(
+                [&](int q) { return q >= Q0 ? j + 1 + (q - Q0) * NB8 : (q == Q0 - 1 && j == NB8 - 1 ? 0 : -1); },
+                [&](int q) { return v[q].x; });
         }
         ep.finish(sp.red_a, sp.red_b, sp.red_f, piece_sums, state);
     }  // frames of this CTA
@@ -457,7 +505,7 @@ template <int F, bool CHAIN>
 __global__ void __launch_bounds__(kConvGlobalThreads)
 convolve_global_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                        const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
-                       const float2* __restrict__ h_side, float2* __restrict__ result, float* __restrict__ mid_plane,
+                       const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
                        double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, float2* scratch, int nframes) {
     constexpr int N = 2 * F;
     constexpr int THREADS = kConvGlobalThreads;
@@ -510,8 +558,12 @@ convolve_global_kernel(const float2* __restrict__ x, long long frames, long long
         fft_run<N, -1, THREADS, float, CHAIN>(planes, tw, PlaneLoad<PackedPlanes>{planes}, PlaneStore<PackedPlanes>{planes},
                                               /*first_in_place=*/true, /*last_in_place=*/true);
         __syncthreads();
-        ConvEpilogue<F> ep(result, mid_plane, n0, frames, piece, divisions, bal);
-        for (int o = tid; o < ep.valid; o += THREADS) ep.emit(o, planes.load(F - 1 + o));
+        ConvEpilogue<F> ep(result, loud, n0, frames, piece, divisions, bal);
+        for (int o0 = 0; o0 < ep.valid; o0 += THREADS) {  // (whole warps to the end: append_loud votes per warp)
+            const int o = o0 + tid;
+            if (o < ep.valid) ep.emit(o, planes.load(F - 1 + o));
+            ep.template append_loud<1>([&](int) { return o; }, [&](int) { return planes.load(F - 1 + o).x; });
+        }
         ep.finish(red_a, red_b, red_f, piece_sums, state);
         __syncthreads();  // the frame buffer and the reduction slots serve the CTA's next frame
     }
@@ -521,12 +573,13 @@ template <int F>
 int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,
                       const Workspace& ws, mgb_track_state* state, cudaStream_t stream) {
     const long long T = layout.target_frames;
+    const LoudList loud{ws.loud_values, ws.loud_count, (long long)ws.loud_capacity, ws.result_slot};
     if constexpr (F > 8192) {
         const int nframes = (int)((T + F - 1) / F);
         auto kernel = g_twiddle_chain ? convolve_global_kernel<F, true> : convolve_global_kernel<F, false>;
         return launch("convolve_kernel", kernel, dim3(conv_global_ctas(F, T)), dim3(kConvGlobalThreads), 0, stream, target, T,
                       (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                      (const float2*)ws.h_mid, (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state,
+                      (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
                       ws.conv_scratch, nframes);
     } else {
         const int ovs = conv_frame_ovs(plan.fft_size, layout.target_piece);
@@ -534,14 +587,14 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
             const unsigned nframes = (unsigned)((T + out - 1) / out);
             return launch("convolve_kernel", kernel, dim3(nframes), dim3(threads), smem, stream, target, T,
                           (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state,
+                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
                           g_use_tma);
         };
         auto args2 = [&](auto kernel, int out, int threads, size_t smem) {  // (the fused kernel also takes the frame count)
             const unsigned nframes = (unsigned)((T + out - 1) / out);
             return launch("convolve_kernel", kernel, dim3(nframes), dim3(threads), smem, stream, target, T,
                           (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state,
+                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
                           g_use_tma, (int)nframes);
         };
         if constexpr (InverseRadices<4 * F>::fused) {
@@ -554,12 +607,12 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
                     auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 4, true, true> : convolve_fused_kernel<F, 4, false, true>;
                     return launch("convolve_kernel", kernel, dim3(grid), dim3(4 * F / 16), ConvSmem<4 * F>::kBytes, stream, target, T,
                                   (long long)layout.target_piece, layout.target_divisions, tw4, (const float2*)ws.h_mid,
-                                  (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state, g_use_tma, (int)nframes);
+                                  (const float2*)ws.h_side, result, loud, ws.piece_sums, state, g_use_tma, (int)nframes);
                 }
                 auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 4, true, false> : convolve_fused_kernel<F, 4, false, false>;
                 return launch("convolve_kernel", kernel, dim3(nframes), dim3(4 * F / 16), ConvSmem<4 * F>::kBytes, stream, target, T,
                               (long long)layout.target_piece, layout.target_divisions, tw4, (const float2*)ws.h_mid,
-                              (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state, g_use_tma, (int)nframes);
+                              (const float2*)ws.h_side, result, loud, ws.piece_sums, state, g_use_tma, (int)nframes);
             }
         }
         if constexpr (InverseRadices<2 * F>::fused) {
@@ -570,7 +623,7 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
                     auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 2, true, true> : convolve_fused_kernel<F, 2, false, true>;
                     return launch("convolve_kernel", kernel, dim3(grid), dim3(F / 8), ConvSmem<2 * F>::kBytes, stream, target, T,
                                   (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                                  (const float2*)ws.h_mid, (const float2*)ws.h_side, result, ws.mid_plane, ws.piece_sums, state,
+                                  (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
                                   g_use_tma, (int)nframes);
                 }
                 return args2(g_twiddle_chain ? convolve_fused_kernel<F, 2, true, false> : convolve_fused_kernel<F, 2, false, false>, F, F / 8,

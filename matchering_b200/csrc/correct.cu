@@ -9,8 +9,8 @@
 //
 // The reference rescales result_mid and result after every step; here the coefficients only
 // accumulate in mgb_track_state::gain (a float64 on the device) and each later pass multiplies by
-// it on the fly, so a step costs one read of the float32 mid plane (4 B/frame, L2-resident for
-// ordinary track lengths) instead of three full-array passes.
+// it on the fly.  A step reads only the mid samples loud enough to clip (the convolution's loud
+// lists, kernels.cuh) instead of three full-array passes.
 #include "kernels.cuh"
 #include "tail.cuh"
 
@@ -18,10 +18,7 @@ namespace mgb {
 
 namespace {
 
-// sum over a piece of clip(mid * gain)^2 ; grid = (chunks per piece, pieces).  Pieces start at
-// arbitrary offsets of the float plane, so a chunk is a scalar head, an aligned float4 body and a
-// scalar tail.
-// clip(mid*gain)^2 of four samples: the product and the clip in float32 (the plane is float32
+// clip(mid*gain)^2 of four samples: the product and the clip in float32 (the samples are float32
 // anyway), the squares summed in float64
 __device__ __forceinline__ double clip_sq4(float4 v, float gain) {
     const float a = fminf(1.0f, fmaxf(-1.0f, v.x * gain)), b = fminf(1.0f, fmaxf(-1.0f, v.y * gain));
@@ -33,38 +30,26 @@ __device__ __forceinline__ double clip_sq(float v, float gain) {
     return (double)c * c;
 }
 
+// A later step's per-piece sums of clip(mid*gain)^2 (kernels.cuh: kLoudMid); grid = (chunks per piece, pieces).
+// From the piece's loud list when that is exact: gain^2 * S_quiet + sum over the list of clip(m*gain)^2, with
+// S_quiet = step-0 sum - sum over the list of clip(m)^2 (every term exact in float64: a float squared).  Otherwise
+// (the list overflowed, or quiet samples could clip at this gain) from the result, mid = (L + R) / 2.
 __global__ void __launch_bounds__(256)
-clip_sumsq_kernel(const float* __restrict__ mid, long long piece, int divisions, int step, double eps,
-                  mgb_track_state* __restrict__ state, const double* __restrict__ prev_sums, double* __restrict__ sums) {
+loud_sumsq_kernel(LoudList loud, long long piece, int divisions, int step, double eps, mgb_track_state* __restrict__ state,
+                  const double* __restrict__ step0_sums, const double* __restrict__ prev_sums, double* __restrict__ sums) {
     __shared__ double red[32];
     const long long p = blockIdx.y;
-    const long long per = (piece + gridDim.x - 1) / gridDim.x;
-    const long long lo = p * piece + (long long)blockIdx.x * per;
-    long long hi = lo + per;
-    if (hi > (p + 1) * piece) hi = (p + 1) * piece;
-    if (hi < lo) hi = lo;
-    long long body_lo = (lo + 3) & ~3LL;
-    if (body_lo > hi) body_lo = hi;
-    long long body_hi = hi & ~3LL;
-    if (body_hi < body_lo) body_hi = body_lo;
-    const float4* body = reinterpret_cast<const float4*>(mid + body_lo);
-    const long long nvec = (body_hi - body_lo) >> 2;
-    const long long stride = 4LL * blockDim.x;
-    auto fetch = [&](long long i, float4* v) {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const long long iu = i + (long long)u * blockDim.x;
-            v[u] = iu < nvec ? body[iu] : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    };
-    // the first loads do not depend on the coefficient: they go out before the prologue's chain of
-    // dependent reads, which then costs no extra DRAM round trip
-    float4 v[4];
-    long long i = threadIdx.x;
-    fetch(i, v);
-    float edge_a = 0.0f, edge_b = 0.0f;  // head / tail (< 4 samples each) outside the 16-byte aligned body
-    if ((long long)threadIdx.x < body_lo - lo) edge_a = mid[lo + threadIdx.x];
-    if ((long long)threadIdx.x < hi - body_hi) edge_b = mid[body_hi + threadIdx.x];
+    const long long n = loud.count[p];
+    const bool fits = n <= loud.capacity;
+    // chunk blockIdx.x takes the float4 groups [lo4, hi4) of the row; entries >= n are not part of the list
+    const long long n4 = fits ? (n + 3) / 4 : 0;
+    const long long per4 = (n4 + gridDim.x - 1) / gridDim.x;
+    const long long lo4 = (long long)blockIdx.x * per4;
+    const long long hi4 = lo4 + per4 < n4 ? lo4 + per4 : n4;
+    const float4* row = reinterpret_cast<const float4*>(loud.values + p * loud.capacity);
+    // the first load does not depend on the coefficient: it goes out before the prologue's chain of dependent reads
+    long long i = lo4 + threadIdx.x;
+    float4 v = i < hi4 ? row[i] : make_float4(0.f, 0.f, 0.f, 0.f);
 
     // prologue, identical in every CTA: the previous step's coefficient from its per-piece sums, and
     // the gain accumulated so far (stages.py:161-168 applied lazily)
@@ -76,15 +61,33 @@ clip_sumsq_kernel(const float* __restrict__ mid, long long piece, int divisions,
         state->steps_done = step;
     }
     const float gain_f = (float)gain;
-    double acc = (double)0.0;
-    acc += clip_sq(edge_a, gain_f) + clip_sq(edge_b, gain_f);  // (zero where there is no edge sample)
-    while (i < nvec) {
-        float4 w[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) w[u] = v[u];
-        i += stride;
-        if (i < nvec) fetch(i, v);  // next batch in flight while this one is reduced
-        acc += (clip_sq4(w[0], gain_f) + clip_sq4(w[1], gain_f)) + (clip_sq4(w[2], gain_f) + clip_sq4(w[3], gain_f));
+    double acc = 0.0;
+    if (fits && gain * (double)kLoudMid <= 1.0 - kLoudMargin) {
+        double loud_g = 0.0, loud_1 = 0.0;
+        while (i < hi4) {
+            float4 w = v;
+            const long long e = 4 * i;  // entry of w.x (< n)
+            i += blockDim.x;
+            if (i < hi4) v = row[i];  // next group in flight while this one is reduced
+            if (e + 1 >= n) w.y = 0.0f;
+            if (e + 2 >= n) w.z = 0.0f;
+            if (e + 3 >= n) w.w = 0.0f;
+            loud_g += clip_sq4(w, gain_f);
+            loud_1 += clip_sq4(w, 1.0f);
+        }
+        // the quiet samples cannot clip: their part is gain^2 * S_quiet, in float64
+        acc = loud_g - gain * gain * loud_1;
+        if (blockIdx.x == 0 && threadIdx.x == 0) acc += gain * gain * step0_sums[p];
+    } else {
+        const float2* res = *loud.result_slot;
+        const long long per = (piece + gridDim.x - 1) / gridDim.x;
+        const long long lo = p * piece + (long long)blockIdx.x * per;
+        const long long hi = lo + per < (p + 1) * piece ? lo + per : (p + 1) * piece;
+#pragma unroll 4
+        for (long long f = lo + threadIdx.x; f < hi; f += blockDim.x) {
+            const float2 x = res[f];
+            acc += clip_sq((x.x + x.y) * 0.5f, gain_f);
+        }
     }
     const double total = block_sum(acc, red);
     if (threadIdx.x == 0 && total != 0.0) atomicAdd(&sums[p], total);
@@ -299,15 +302,18 @@ unsigned grid_for(long long items, int per_block) {
 
 }  // namespace
 
-int launch_clip_sumsq(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws, int step,
+int launch_loud_sumsq(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws, int step,
                       mgb_track_state* state, cudaStream_t stream) {
+    // The grid is fixed before the device decides between list and result, so it is sized for a pass over
+    // the result (three CTAs per SM); a list, at most a quarter of the piece, leaves most of them a few entries.
     const int div = layout.target_divisions;
-    long long per_piece = ((long long)g_clip_ctas_per_sm * num_sms() + div - 1) / div;
+    long long per_piece = (3LL * num_sms() + div - 1) / div;
     const long long max_useful = (layout.target_piece + 8191) / 8192;
     if (per_piece > max_useful) per_piece = max_useful;
     if (per_piece < 1) per_piece = 1;
-    return launch("clip_sumsq_kernel", clip_sumsq_kernel, dim3((unsigned)per_piece, (unsigned)div), dim3(256), 0, stream,
-                  (const float*)ws.mid_plane, (long long)layout.target_piece, div, step, plan.min_value, state,
+    const LoudList loud{ws.loud_values, ws.loud_count, (long long)ws.loud_capacity, ws.result_slot};
+    return launch("loud_sumsq_kernel", loud_sumsq_kernel, dim3((unsigned)per_piece, (unsigned)div), dim3(256), 0, stream, loud,
+                  (long long)layout.target_piece, div, step, plan.min_value, state, (const double*)ws.piece_sums,
                   (const double*)(ws.piece_sums + (long long)(step - 1) * div), ws.piece_sums + (long long)step * div);
 }
 

@@ -17,12 +17,15 @@ struct Workspace {
     double* design;         // [2 channels][4 CTAs][design_stride] float64 vectors of the FIR design
     float2* h_mid;          // [2F+1] spectrum of the mid FIR on the convolution's N = 2F or 4F grid (bins 0..N/2), c0/N folded in
     float2* h_side;         // [2F+1]
-    float* mid_plane;       // [T] mid channel of the convolution result
+    float* loud_values;     // [Dt][loud_capacity] counted mid samples of the convolution result with |mid| >= kLoudMid, per piece
+    const float2** result_slot;  // device address of the convolution's result, recorded by the convolution kernel
     float2* conv_scratch;   // fft_size 16384 only: one padded 2F-point frame per CTA of convolve_global_kernel
     // ---- zeroed at the start of every job (one memset) ----
     unsigned char* zero_begin;
     double* piece_sums;     // [MGB_MAX_CORRECTION_STEPS][Dt] sums of clip(mid*gain)^2
+    unsigned* loud_count;   // [Dt] appends to each piece's loud list (may exceed loud_capacity: the list overflowed)
     unsigned char* zero_end;
+    int64_t loud_capacity;  // entries per piece
     // ---- zeroed before every limiter launch (limiter_zero_bytes from `tickets` on) ----
     int* tickets;           // [64] zeroed counters: 0 = limiter chunk ticket
     unsigned char* lookback;// [nchunks] LookbackSlot
@@ -66,6 +69,26 @@ constexpr int kLimiterCoreEpt = 9;                                   // core sam
 constexpr int kLimiterCore = kLimiterThreads * kLimiterCoreEpt;      // 4608 samples per chunk
 constexpr int kLimiterSpanEptMax = 25;                               // span samples per thread (odd): up to 8192 samples of halo (215 KB of shared memory)
 
+// RMS-correction steps 2..n from loud lists.  The convolution's epilogue appends every counted mid sample m with
+// |m| >= kLoudMid to its piece's loud list; all other samples ("quiet") enter the later steps only through
+// S_quiet = (step-0 sum) - sum over the list of clip(m)^2.  A later step at accumulated gain g takes
+// g^2 S_quiet + sum over the list of clip(m*g)^2, which is exact as long as no quiet sample can clip:
+// g * kLoudMid <= 1 - kLoudMargin (the margin covers the float32 rounding of the gain and the product).
+// Otherwise, or when a piece's list overflowed, the step re-reads that piece of the result instead.
+// 0.5 keeps the list exact up to 6 dB of correction (the benchmark tracks need at most 0.2 dB); 12-13 % of
+// the samples of the c2 benchmark tracks are that loud, 5 % of c3's (11 % in its loudest piece), so a
+// capacity of a quarter of the piece leaves room for twice that.
+constexpr float kLoudMid = 0.5f;
+constexpr double kLoudMargin = 1e-6;
+inline int64_t loud_capacity(int64_t piece) { return ((piece + 3) / 4 + 3) / 4 * 4; }  // a multiple of 4: float4 rows
+
+struct LoudList {
+    float* values;
+    unsigned* count;
+    long long capacity;
+    const float2** result_slot;
+};
+
 Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& layout, void* base);
 int64_t limiter_lookback_bytes(const mgb_limiter_params& lp, int64_t frames);
 int64_t limiter_tables_bytes();
@@ -90,7 +113,7 @@ int launch_convolve(const mgb_plan& plan, const mgb_track_layout& layout, const 
 // correct.cu ------------------------------------------------------------------------------------
 int launch_correction_final(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws,
                             mgb_track_state* state, cudaStream_t stream);
-int launch_clip_sumsq(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws, int step,
+int launch_loud_sumsq(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws, int step,
                       mgb_track_state* state, cudaStream_t stream);
 int launch_scale(const float2* in, float2* out, int64_t frames, const double* gain, const double* divisor,
                  cudaStream_t stream);
@@ -125,7 +148,6 @@ extern int g_use_tma;
 bool host_set_option(const char* name, int value);  // hostio.cu: the host transport's tuning switches
 extern int g_limiter_ticket;      // limiter chunks by atomic ticket (1) or by block index (0, default)
 extern int g_lookback_inclusive;  // limiter chunks publish their inclusive state (1, default) or aggregates only (0, tests)
-extern int g_clip_ctas_per_sm;  // grid of the correction passes, in CTAs per SM (tuning switch)
 extern int g_conv_ovs;       // convolution: FIR lengths per overlap-save frame where the long-frame kernel exists (4, default) or 2
 extern int g_conv_fused;     // convolution: ends of both transforms in registers where the schedule allows (1)
 extern int g_conv_persistent;  // convolution (16384-point frames): one CTA per SM walks its frames, next frame's bulk copy under the epilogue

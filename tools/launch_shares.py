@@ -6,7 +6,7 @@ import sys
 from collections import defaultdict
 
 PIPELINE = ("analyze_kernel", "spectrum_mean_kernel", "smooth_operator_kernel", "design_kernel", "convolve",
-            "clip_sumsq_kernel", "correction_final_kernel", "limiter_kernel")
+            "loud_sumsq_kernel", "correction_final_kernel", "limiter_kernel")
 
 steps = int(sys.argv[3]) if len(sys.argv) > 3 else 3
 rows = [r for r in csv.reader(l for l in open(sys.argv[1]) if l.startswith('"'))]
