@@ -377,6 +377,10 @@ int mgb_test_limiter_gains(const mgb_limiter_params* params, const float* d_in_l
  * (target mid, target side, reference mid, reference side), already scaled. d_fir_out [2][F]. */
 int mgb_test_design_fir(const mgb_plan* plan, const double* d_avg, double* d_fir_out, void* d_workspace,
                         void* stream);
+/* where the stages leave their hand-off values in a job's workspace: out[0..12] = byte offsets from d_workspace of
+ * spec_part_t, spec_part_r, sumsq_part_t, sumsq_part_r, absmax_part_t, absmax_part_r, mask_t, mask_r, h_mid, h_side,
+ * loud_values, piece_sums, loud_count; out[13] = loud_capacity (entries per piece); out[14..15] = 0. */
+int mgb_test_workspace_regions(const mgb_plan* plan, const mgb_track_layout* layout, int64_t out[16]);
 
 #ifdef __cplusplus
 }

@@ -183,6 +183,7 @@ PROTOTYPES = {
     "mgb_test_fft": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                C.c_void_p]),
     "mgb_test_design_fir": (C.c_int, [C.POINTER(Plan), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mgb_test_workspace_regions": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.POINTER(C.c_int64)]),
 }
 
 

@@ -79,12 +79,13 @@ int num_sms() {
 
 static inline int64_t align256(int64_t v) { return (v + 255) / 256 * 256; }
 
+// With base_ptr == nullptr every pointer of the result holds its region's byte offset (mgb_test_workspace_regions).
 Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void* base_ptr) {
     Workspace w;
-    unsigned char* base = reinterpret_cast<unsigned char*>(base_ptr);
+    const uintptr_t base = reinterpret_cast<uintptr_t>(base_ptr);
     int64_t off = 0;
     auto take = [&](int64_t bytes) {
-        unsigned char* p = base ? base + off : nullptr;
+        unsigned char* p = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
         off += align256(bytes);
         return p;
     };
@@ -107,10 +108,10 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     w.loud_values = (float*)take(w.loud_capacity * L.target_divisions * 4);
     w.result_slot = (const float2**)take(8);
     w.conv_scratch = (float2*)take(conv_global_scratch_bytes(plan.fft_size, L.target_frames));
-    w.zero_begin = base ? base + off : nullptr;
+    w.zero_begin = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
     w.piece_sums = (double*)take((int64_t)MGB_MAX_CORRECTION_STEPS * L.target_divisions * 8);
     w.loud_count = (unsigned*)take((int64_t)L.target_divisions * 4);
-    w.zero_end = base ? base + off : nullptr;
+    w.zero_end = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
     // zeroed by mgb_finalize right before every limiter launch (a second finalize on the same track
     // must not find the first one's tickets and published carries)
     const int64_t limiter_zero_from = off;
@@ -711,6 +712,19 @@ int mgb_test_fft(int32_t n, int32_t is_f64, int32_t dir, const void* d_in, void*
                  const void* d_twiddles, void* stream) {
     MGB_REQUIRE(d_in && d_out && d_twiddles && batch > 0, MGB_ERR_INVALID, "test_fft: bad arguments");
     return launch_test_fft(n, is_f64, dir, d_in, d_out, batch, d_twiddles, (cudaStream_t)stream);
+}
+
+int mgb_test_workspace_regions(const mgb_plan* plan, const mgb_track_layout* layout, int64_t out[16]) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(layout != nullptr && out != nullptr, MGB_ERR_INVALID, "test_workspace_regions: NULL argument");
+    const Workspace w = carve_workspace(*plan, *layout, nullptr);  // pointers = byte offsets
+    const void* regions[13] = {w.spec_part_t, w.spec_part_r, w.sumsq_part_t, w.sumsq_part_r, w.absmax_part_t,
+                               w.absmax_part_r, w.mask_t, w.mask_r, w.h_mid, w.h_side, w.loud_values, w.piece_sums,
+                               w.loud_count};
+    for (int i = 0; i < 16; ++i) out[i] = 0;
+    for (int i = 0; i < 13; ++i) out[i] = (int64_t)reinterpret_cast<uintptr_t>(regions[i]);
+    out[13] = w.loud_capacity;
+    return MGB_OK;
 }
 
 int mgb_test_design_fir(const mgb_plan* plan, const double* d_avg, double* d_fir_out, void* d_workspace, void* stream) {
