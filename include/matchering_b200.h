@@ -103,7 +103,7 @@ typedef struct mgb_plan {
     void* d_tw_f32_F;    /* float2  table of the F-point transform  */
     void* d_tw_f32_2F;   /* float2  table of the 2F-point transform */
     void* d_tw_f64_F;    /* double2 table of the F-point transform  */
-    void* d_tw_f64_2F;   /* double2 table of the 2F-point transform */
+    void* d_tw_f64_2F;   /* double2 table of the 2F-point transform (then the 4F-point one for fft_size 2048, 4096) */
     void* d_limiter_tables; /* powers of the limiter's three poles (blocked-scan carries) */
     /* optional: the whole smoothing chain (spline, LOWESS, spline, overrides) as one Config-only matrix,
      * s = S m, S [n_lin][n_lin].  mgb_plan_build_operator builds it densely on the device; it is numerically
@@ -135,7 +135,8 @@ typedef struct mgb_track_state {
     int32_t steps_done;
     float fir_peak_mid_bits;      /* max |H_mid[k]| of the designed FIR spectrum (as applied)         */
     float fir_peak_side_bits;     /* max |H_side[k]|                                                  */
-    int32_t reserved;
+    int32_t conv_precise;         /* 1 when the convolution ran with float64 transforms (FIR gain x target peak too
+                                     large for float32 frames, convolve.cu), 0 otherwise                       */
 } mgb_track_state;
 
 /* Geometry of one mastering job, computed by mgb_track_layout from sizes + plan (host side). */

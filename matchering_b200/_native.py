@@ -98,7 +98,7 @@ class TrackState(C.Structure):
         ("steps_done", C.c_int32),
         ("fir_peak_mid_bits", C.c_float),
         ("fir_peak_side_bits", C.c_float),
-        ("reserved", C.c_int32),
+        ("conv_precise", C.c_int32),
     ]
 
 

@@ -107,6 +107,7 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     w.loud_capacity = loud_capacity(L.target_piece);
     w.loud_values = (float*)take(w.loud_capacity * L.target_divisions * 4);
     w.result_slot = (const float2**)take(8);
+    w.target_peak = (float*)take(4);
     w.conv_scratch = (float2*)take(conv_global_scratch_bytes(plan.fft_size, L.target_frames));
     w.zero_begin = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
     w.piece_sums = (double*)take((int64_t)MGB_MAX_CORRECTION_STEPS * L.target_divisions * 8);
@@ -385,7 +386,8 @@ int mgb_plan_twiddle_bytes(int32_t fft_size, int64_t bytes_out[5]) {
     bytes_out[0] = (int64_t)cf * 8;
     bytes_out[1] = (int64_t)(c2 + inverse_twiddle_count(2 * fft_size) + long_frame_twiddle_count(fft_size)) * 8;
     bytes_out[2] = (int64_t)cf * 16;
-    bytes_out[3] = (int64_t)c2 * 16;
+    // the convolution's float64 tables (convolve_precise_kernel): 2F points, and 4F behind them where 4F frames exist
+    bytes_out[3] = (int64_t)(c2 + (long_frame_twiddle_count(fft_size) ? twiddle_count(4 * fft_size) : 0)) * 16;
     bytes_out[4] = limiter_tables_bytes();
     return MGB_OK;
 }
@@ -405,7 +407,11 @@ int mgb_plan_fill_twiddles(const mgb_plan* plan, void* stream) {
         MGB_TRY(fill_inverse_twiddles(4 * plan->fft_size, tw4, st));
     }
     MGB_TRY(fill_twiddles(plan->fft_size, 1, plan->d_tw_f64_F, st));
-    if (plan->d_tw_f64_2F && plan->fft_size <= 4096) MGB_TRY(fill_twiddles(2 * plan->fft_size, 1, plan->d_tw_f64_2F, st));
+    if (plan->d_tw_f64_2F) {
+        MGB_TRY(fill_twiddles(2 * plan->fft_size, 1, plan->d_tw_f64_2F, st));
+        if (long_frame_twiddle_count(plan->fft_size))
+            MGB_TRY(fill_twiddles(4 * plan->fft_size, 1, (cpx<double>*)plan->d_tw_f64_2F + twiddle_count(2 * plan->fft_size), st));
+    }
     if (!plan->d_limiter_tables) return MGB_OK;  // FFT-only plans (tests); mgb_finalize insists on the tables
     MGB_TRY(check_aligned(plan->d_limiter_tables, "d_limiter_tables"));
     return launch_limiter_tables(plan->limiter, plan->d_limiter_tables, st);

@@ -45,6 +45,32 @@ struct ConvFirst {
     }
 };
 
+// ---- float32 or float64 transforms -----------------------------------------------------------------
+// A float32 transform's rounding noise is spread over all N bins, relative to the frame's norm.  The FIR spectrum
+// scales every bin by its gain, also the bins where the target has no content, and the inverse transform spreads
+// the product over the frame's outputs, before a transient as much as after it.  An output sample's error is then
+// about u sqrt(log2 N) (a random walk over the passes) times max|c0 H| (the largest gain of the FIR as applied)
+// times the frame's level, which max|target| bounds; on band-limited and transient material the ratio of the
+// measured error to that estimate stayed below 0.9.  Broadband material has gains near 20 (the benchmark's
+// 3-minute tracks: 23, an estimate of 2.6e-6, measured errors below 1e-6).  A dull or band-limited target matched to a
+// bright reference has gains of 300 to 10^4 in its empty band, and the float32 result misses the 1e-5 parity
+// bound by up to 10x.  Where the estimate exceeds kConvPreciseError, half that bound, the track is convolved with
+// float64 transforms (convolve_precise_kernel, rounding noise 2^-53 instead of 2^-24).  The choice comes from the
+// track state the design kernel leaves (both FIR peaks) and the target's peak (Workspace::target_peak, from
+// spectrum_mean_kernel): every convolution kernel evaluates the same products, the float32 kernels return at once
+// where it says float64, and the float64 kernel, launched after them for every track, returns at once otherwise;
+// the float64 kernel records the choice in mgb_track_state::conv_precise.
+constexpr double kConvPreciseError = 5e-6;
+template <int N>
+__device__ __forceinline__ bool conv_precise(const mgb_track_state* __restrict__ state, const float* __restrict__ target_peak) {
+    constexpr int kLog2N = N == 1024 ? 10 : N == 2048 ? 11 : N == 4096 ? 12 : N == 8192 ? 13 : N == 16384 ? 14 : 15;
+    static_assert((1 << kLog2N) == N, "frame length");
+    // (products only, the same in every kernel: no contraction can make two kernels disagree)
+    const double e = 0x1p-24 * (double)N * (double)fmaxf(state->fir_peak_mid_bits, state->fir_peak_side_bits) *
+                     (double)*target_peak;
+    return e * e * (double)kLog2N > kConvPreciseError * kConvPreciseError;
+}
+
 // ---- shared by both kernels: frame load + channel balance, FIR spectra on a pair, the epilogue -----
 struct ConvBalance {
     float inv_g;
@@ -214,6 +240,20 @@ struct ConvEpilogue {
             }
         }
     }
+    // emit() from a float64 transform (convolve_precise_kernel): L and R rounded once each, from mid +- side
+    __device__ __forceinline__ void emit_wide(int o, cpx<double> y) {
+        if (o < valid) {
+            const double md = mid_silent ? 0.0 : y.x, sd = side_silent ? 0.0 : y.y;
+            const float m = (float)md, l = (float)(md + sd), r = (float)(md - sd);
+            res[o] = make_float2(l, r);
+            peak = fmaxf(peak, fmaxf(fabsf(l), fabsf(r)));
+            if (o < count_to) {
+                const float cf = fminf(1.0f, fmaxf(-1.0f, m));  // dsp.clip
+                const double c2 = (double)cf * (double)cf;
+                if (o < boundary) sq_a += c2; else sq_b += c2;
+            }
+        }
+    }
     // Appends the loud ones among K outputs per thread to the loud lists: outputs(k) is the k-th output's
     // index o (< 0: none), mids(k) its transform value's real part.  Every lane of the warp calls, with
     // the same K; per warp and piece one atomicAdd reserves the room for all K.  Entries past a list's
@@ -311,9 +351,10 @@ __global__ void __launch_bounds__(F / 8, (F <= 4096 ? 2 : 1))
 convolve_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                 const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
                 const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
-                double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, int use_tma) {
+                double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, const float* __restrict__ target_peak, int use_tma) {
     constexpr int N = 2 * F;
     constexpr int THREADS = N / 16;
+    if (conv_precise<N>(state, target_peak)) return;  // convolve_precise_kernel's track
     MGB_DYN_SMEM(smem);
     const ConvPointers<N> sp(smem);
     const PackedPlanes planes = sp.planes;
@@ -380,7 +421,7 @@ __global__ void __launch_bounds__(OVS * F / 16, (OVS * F <= 8192 ? 2 : 1))
 convolve_fused_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                       const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
                       const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
-                      double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, int use_tma, int nframes) {
+                      double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, const float* __restrict__ target_peak, int use_tma, int nframes) {
     constexpr int N = OVS * F;
     constexpr int OUT = N - F;  // outputs per frame
     constexpr int THREADS = N / 16;
@@ -392,6 +433,7 @@ convolve_fused_kernel(const float2* __restrict__ x, long long frames, long long 
     static_assert(fft_last_pass_ns<Fwd>() == NB8 && fft_last_pass_ns<Inv>() == NB8 && NB8 == 2 * THREADS, "schedule");
     static_assert(Q0 * NB8 == F && Q0 >= 1 && Q0 < 8, "frame length");
     const cpx<float>* tw_inv = tw + fft_schedule_twiddles<Fwd>();
+    if (conv_precise<N>(state, target_peak)) return;  // convolve_precise_kernel's track
     MGB_DYN_SMEM(smem);
     const ConvPointers<N> sp(smem);
     const PackedPlanes planes = sp.planes;
@@ -506,12 +548,13 @@ __global__ void __launch_bounds__(kConvGlobalThreads)
 convolve_global_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
                        const cpx<float>* __restrict__ tw, const float2* __restrict__ h_mid,
                        const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
-                       double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, float2* scratch, int nframes) {
+                       double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, const float* __restrict__ target_peak, float2* scratch, int nframes) {
     constexpr int N = 2 * F;
     constexpr int THREADS = kConvGlobalThreads;
     __shared__ double red_a[32], red_b[32];
     __shared__ float red_f[32];
     __shared__ unsigned red_u[2];
+    if (conv_precise<N>(state, target_peak)) return;  // convolve_precise_kernel's track
     const PackedPlanes planes{scratch + (long long)blockIdx.x * PackedPlanes::elems(N)};
     const int tid = threadIdx.x;
     for (int frame = blockIdx.x; frame < nframes; frame += gridDim.x) {
@@ -569,9 +612,136 @@ convolve_global_kernel(const float2* __restrict__ x, long long frames, long long
     }
 }
 
+// ---- float64 transforms, for the tracks conv_precise picks ----------------------------------------------
+// The same overlap-save frames as the float32 kernel of the track (N = OVS*F points, OUT = N - F outputs, the FIR
+// spectra on the same grid), transformed in float64: mid and side formed exactly from L and R, one complex
+// transform for both (no balancing: float64 noise is 2^-29 of float32's), the product with the float32 FIR
+// spectra in float64, and L, R = mid +- side rounded once each.  Each CTA keeps its frame as two padded float64
+// planes in a workspace region (L2-resident) and walks the frames blockIdx.x, blockIdx.x + gridDim.x, ...;
+// the epilogue (per-piece sums, loud lists, peak) is the float32 kernels' own.  Not tuned: correct first.
+constexpr int kConvPreciseThreads = 512;
+template <int F, int OVS>
+__global__ void __launch_bounds__(kConvPreciseThreads, 1)
+convolve_precise_kernel(const float2* __restrict__ x, long long frames, long long piece, int divisions,
+                        const cpx<double>* __restrict__ tw, const float2* __restrict__ h_mid,
+                        const float2* __restrict__ h_side, float2* __restrict__ result, LoudList loud,
+                        double* __restrict__ piece_sums, mgb_track_state* __restrict__ state, const float* __restrict__ target_peak, double* scratch, int nframes) {
+    constexpr int N = OVS * F;
+    constexpr int OUT = N - F;
+    constexpr int THREADS = kConvPreciseThreads;
+    using Planes = SplitPlanes<double>;
+    __shared__ double red_a[32], red_b[32];
+    __shared__ float red_f[32];
+    __shared__ unsigned red_u[2];
+    if (!conv_precise<N>(state, target_peak)) return;  // the float32 kernel's track
+    if (blockIdx.x == 0 && threadIdx.x == 0) state->conv_precise = 1;
+    double* re = scratch + (long long)blockIdx.x * 2 * Planes::elems(N);
+    const Planes planes{re, re + Planes::elems(N)};
+    const int tid = threadIdx.x;
+    for (int frame = blockIdx.x; frame < nframes; frame += gridDim.x) {
+        const long long n0 = (long long)frame * OUT;
+        const long long origin = n0 - F / 2;
+        const ConvSpan span = conv_span<N>(frames, origin);
+        ConvFirst first;
+        first.raw = x + origin;  // (only indices inside [lo, hi) are dereferenced)
+        first.lo = (int)(span.lo - origin);
+        first.hi = (int)(span.hi - origin);
+        first.fixup = nullptr;
+        first.fix_index = -1;
+        // which channels are exactly silent in this frame (they stay so, as in the reference)
+        float max_mid = 0.0f, max_side = 0.0f;
+        for (int i = tid; i < N; i += THREADS) {
+            const float2 v = first.sample(i);
+            max_mid = fmaxf(max_mid, fabsf(v.x + v.y));
+            max_side = fmaxf(max_side, fabsf(v.x - v.y));
+        }
+        if (tid == 0) red_u[0] = red_u[1] = 0u;
+        __syncthreads();
+        block_max2(max_mid, max_side, red_u);
+        ConvBalance bal;
+        bal.inv_g = 1.0f;
+        bal.mid_silent = max_mid == 0.0f;
+        bal.side_silent = max_side == 0.0f;
+        bal.any_silent = bal.mid_silent || bal.side_silent;
+        auto z_of = [&](int i) {  // (L +- R)/2 of two floats is exact in float64
+            const float2 v = first.sample(i);
+            return cpx<double>{0.5 * ((double)v.x + (double)v.y), 0.5 * ((double)v.x - (double)v.y)};
+        };
+        fft_run<N, +1, THREADS, double>(planes, tw, z_of, PlaneStore<Planes>{planes}, /*first_in_place=*/false,
+                                        /*last_in_place=*/true);
+        __syncthreads();
+        for (int k = tid; k <= N / 2; k += THREADS) {
+            const int kn = (N - k) & (N - 1);
+            const cpx<double> zk = planes.load(k), zn = planes.load(kn);
+            // M = (Z[k] + conj Z[N-k])/2 ; S = (Z[k] - conj Z[N-k])/(2i)
+            const double mr = 0.5 * (zk.x + zn.x), mi = 0.5 * (zk.y - zn.y);
+            const double sr = 0.5 * (zk.y + zn.y), si = 0.5 * (zn.x - zk.x);
+            const float2 hm = h_mid[k], hs = h_side[k];
+            double pmr = hm.x * mr - hm.y * mi, pmi = hm.x * mi + hm.y * mr;
+            double psr = hs.x * sr - hs.y * si, psi = hs.x * si + hs.y * sr;
+            if (bal.mid_silent) pmr = pmi = 0.0;
+            if (bal.side_silent) psr = psi = 0.0;
+            planes.store(k, cpx<double>{pmr - psi, pmi + psr});
+            if (kn != k) planes.store(kn, cpx<double>{pmr + psi, psr - pmi});
+        }
+        __syncthreads();
+        fft_run<N, -1, THREADS, double>(planes, tw, PlaneLoad<Planes>{planes}, PlaneStore<Planes>{planes},
+                                        /*first_in_place=*/true, /*last_in_place=*/true);
+        __syncthreads();
+        ConvEpilogue<OUT> ep(result, loud, n0, frames, piece, divisions, bal);
+        for (int o0 = 0; o0 < ep.valid; o0 += THREADS) {  // (whole warps to the end: append_loud votes per warp)
+            const int o = o0 + tid;
+            if (o < ep.valid) ep.emit_wide(o, planes.load(F - 1 + o));
+            ep.template append_loud<1>([&](int) { return o; }, [&](int) { return (float)planes.load(F - 1 + o).x; });
+        }
+        ep.finish(red_a, red_b, red_f, piece_sums, state);
+        __syncthreads();  // the frame's planes and the reduction slots serve the CTA's next frame
+    }
+}
+
+// frame length (points) and CTAs of the float64 convolution, whose planes share the workspace region of
+// convolve_global_kernel's frames (the two never run on the same track)
+static int conv_precise_points(int fft_size) { return (fft_size == 2048 || fft_size == 4096) ? 4 * fft_size : 2 * fft_size; }
+static int conv_precise_ctas(int fft_size, long long target_frames) {
+    const long long nframes = (target_frames + fft_size - 1) / fft_size;  // (at least as many as any OVS needs)
+    return (int)(nframes < num_sms() ? nframes : num_sms());
+}
+
+template <int F, int OVS>
+int launch_convolve_precise(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,
+                            const Workspace& ws, mgb_track_state* state, cudaStream_t stream) {
+    MGB_REQUIRE(plan.d_tw_f64_2F != nullptr, MGB_ERR_INVALID, "convolve: d_tw_f64_2F is NULL");
+    const long long T = layout.target_frames;
+    const LoudList loud{ws.loud_values, ws.loud_count, (long long)ws.loud_capacity, ws.result_slot};
+    const int nframes = (int)((T + (OVS - 1) * F - 1) / ((OVS - 1) * F));
+    const int ctas = conv_precise_ctas(F, T);
+    // the 4F-point table lives behind the 2F-point one (mgb_plan_twiddle_bytes)
+    const cpx<double>* tw = (const cpx<double>*)plan.d_tw_f64_2F + (OVS == 4 ? twiddle_count(2 * F) : 0);
+    return launch("convolve_precise_kernel", convolve_precise_kernel<F, OVS>, dim3(nframes < ctas ? nframes : ctas),
+                  dim3(kConvPreciseThreads), 0, stream, target, T, (long long)layout.target_piece, layout.target_divisions,
+                  tw, (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak,
+                  (double*)ws.conv_scratch, nframes);
+}
+
+template <int F>
+int launch_convolve_f32(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,
+                        const Workspace& ws, mgb_track_state* state, cudaStream_t stream);
+
+// the float32 kernel, then the float64 one: on every track one of the two returns at once (conv_precise)
 template <int F>
 int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,
                       const Workspace& ws, mgb_track_state* state, cudaStream_t stream) {
+    MGB_TRY(launch_convolve_f32<F>(plan, layout, target, result, ws, state, stream));
+    if constexpr (F == 2048 || F == 4096) {
+        if (conv_frame_ovs(plan.fft_size, layout.target_piece) == 4)
+            return launch_convolve_precise<F, 4>(plan, layout, target, result, ws, state, stream);
+    }
+    return launch_convolve_precise<F, 2>(plan, layout, target, result, ws, state, stream);
+}
+
+template <int F>
+int launch_convolve_f32(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,
+                        const Workspace& ws, mgb_track_state* state, cudaStream_t stream) {
     const long long T = layout.target_frames;
     const LoudList loud{ws.loud_values, ws.loud_count, (long long)ws.loud_capacity, ws.result_slot};
     if constexpr (F > 8192) {
@@ -579,7 +749,7 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
         auto kernel = g_twiddle_chain ? convolve_global_kernel<F, true> : convolve_global_kernel<F, false>;
         return launch("convolve_kernel", kernel, dim3(conv_global_ctas(F, T)), dim3(kConvGlobalThreads), 0, stream, target, T,
                       (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                      (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
+                      (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak,
                       ws.conv_scratch, nframes);
     } else {
         const int ovs = conv_frame_ovs(plan.fft_size, layout.target_piece);
@@ -587,14 +757,14 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
             const unsigned nframes = (unsigned)((T + out - 1) / out);
             return launch("convolve_kernel", kernel, dim3(nframes), dim3(threads), smem, stream, target, T,
                           (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
+                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak,
                           g_use_tma);
         };
         auto args2 = [&](auto kernel, int out, int threads, size_t smem) {  // (the fused kernel also takes the frame count)
             const unsigned nframes = (unsigned)((T + out - 1) / out);
             return launch("convolve_kernel", kernel, dim3(nframes), dim3(threads), smem, stream, target, T,
                           (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
+                          (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak,
                           g_use_tma, (int)nframes);
         };
         if constexpr (InverseRadices<4 * F>::fused) {
@@ -607,12 +777,12 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
                     auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 4, true, true> : convolve_fused_kernel<F, 4, false, true>;
                     return launch("convolve_kernel", kernel, dim3(grid), dim3(4 * F / 16), ConvSmem<4 * F>::kBytes, stream, target, T,
                                   (long long)layout.target_piece, layout.target_divisions, tw4, (const float2*)ws.h_mid,
-                                  (const float2*)ws.h_side, result, loud, ws.piece_sums, state, g_use_tma, (int)nframes);
+                                  (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak, g_use_tma, (int)nframes);
                 }
                 auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 4, true, false> : convolve_fused_kernel<F, 4, false, false>;
                 return launch("convolve_kernel", kernel, dim3(nframes), dim3(4 * F / 16), ConvSmem<4 * F>::kBytes, stream, target, T,
                               (long long)layout.target_piece, layout.target_divisions, tw4, (const float2*)ws.h_mid,
-                              (const float2*)ws.h_side, result, loud, ws.piece_sums, state, g_use_tma, (int)nframes);
+                              (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak, g_use_tma, (int)nframes);
             }
         }
         if constexpr (InverseRadices<2 * F>::fused) {
@@ -623,7 +793,7 @@ int launch_convolve_t(const mgb_plan& plan, const mgb_track_layout& layout, cons
                     auto kernel = g_twiddle_chain ? convolve_fused_kernel<F, 2, true, true> : convolve_fused_kernel<F, 2, false, true>;
                     return launch("convolve_kernel", kernel, dim3(grid), dim3(F / 8), ConvSmem<2 * F>::kBytes, stream, target, T,
                                   (long long)layout.target_piece, layout.target_divisions, (const cpx<float>*)plan.d_tw_f32_2F,
-                                  (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state,
+                                  (const float2*)ws.h_mid, (const float2*)ws.h_side, result, loud, ws.piece_sums, state, ws.target_peak,
                                   g_use_tma, (int)nframes);
                 }
                 return args2(g_twiddle_chain ? convolve_fused_kernel<F, 2, true, false> : convolve_fused_kernel<F, 2, false, false>, F, F / 8,
@@ -644,7 +814,10 @@ int conv_global_ctas(int fft_size, long long target_frames) {
     return (int)(nframes < cap ? nframes : cap);
 }
 int64_t conv_global_scratch_bytes(int fft_size, long long target_frames) {
-    return (int64_t)conv_global_ctas(fft_size, target_frames) * (int64_t)PackedPlanes::bytes(2 * fft_size);
+    const int64_t global = (int64_t)conv_global_ctas(fft_size, target_frames) * (int64_t)PackedPlanes::bytes(2 * fft_size);
+    const int64_t precise = (int64_t)conv_precise_ctas(fft_size, target_frames) *
+                            (int64_t)SplitPlanes<double>::bytes(conv_precise_points(fft_size));
+    return global > precise ? global : precise;
 }
 
 // Overlap-save frame length, in FIR lengths, of the convolution (and therefore the grid the design kernel

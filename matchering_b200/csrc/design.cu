@@ -316,6 +316,8 @@ struct DesignArgs {
     const float* spec_part_r;
     unsigned char* mask_t;  // global copies of the loudest-piece masks (written for inspection)
     unsigned char* mask_r;
+    const float* absmax_t;       // [div_t*slots_t + 1] the target's peaks per (piece, slot) and of its tail
+    float* target_peak;          // out: their maximum (Workspace::target_peak)
     LevelsArgs levels;
     int div_t, slots_t, div_r, slots_r;
     long long frames_per_piece_t, frames_per_piece_r;
@@ -373,16 +375,22 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
     // serial L2 latency) -- then warp 0 derives the statistics from the per-piece sums with shuffles and leaves
     // the masks and the scalars in shared memory; CTA (0,0) records them in the track state.
     __shared__ LevelsResult lv_s;
-    __shared__ unsigned peak_bits_s;
+    __shared__ unsigned peak_bits_s, target_peak_bits_s;
     double* piece_sum = reinterpret_cast<double*>(smem + ((a.div_t + a.div_r + 15) / 16) * 16);  // [div_t + div_r]
     {
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-        if (threadIdx.x == 0) peak_bits_s = 0u;
+        if (threadIdx.x == 0) peak_bits_s = target_peak_bits_s = 0u;
         __syncthreads();
         float pk = 0.0f;
         for (int i = threadIdx.x; i < a.div_r * a.slots_r + 1; i += blockDim.x) pk = fmaxf(pk, a.levels.absmax_r[i]);
         pk = warp_max_f(pk);
         if (lane == 0 && pk > 0.0f) atomicMax(&peak_bits_s, __float_as_uint(pk));  // non-negative floats order like their bits
+        if (blockIdx.x == 0 && blockIdx.y == 0) {  // the target's peak: the convolution's choice of precision needs it
+            float tpk = 0.0f;
+            for (int i = threadIdx.x; i < a.div_t * a.slots_t + 1; i += blockDim.x) tpk = fmaxf(tpk, a.absmax_t[i]);
+            tpk = warp_max_f(tpk);
+            if (lane == 0 && tpk > 0.0f) atomicMax(&target_peak_bits_s, __float_as_uint(tpk));
+        }
         for (int p = warp; p < a.div_t + a.div_r; p += nwarps) {
             const bool is_t = p < a.div_t;
             const double* part = is_t ? a.levels.sumsq_t + (long long)p * a.slots_t
@@ -414,7 +422,8 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
             a.state->conv_peak_bits = 0.0f;
             a.state->fir_peak_mid_bits = 0.0f;
             a.state->fir_peak_side_bits = 0.0f;
-            a.state->reserved = 0;
+            a.state->conv_precise = 0;
+            *a.target_peak = __uint_as_float(target_peak_bits_s);
         }
         for (int p = threadIdx.x; p < a.div_t; p += blockDim.x) a.mask_t[p] = mask_t[p];
         for (int p = threadIdx.x; p < a.div_r; p += blockDim.x) a.mask_r[p] = mask_r[p];
@@ -741,6 +750,8 @@ int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Wo
     a.spec_part_r = ws.spec_part_r;
     a.mask_t = ws.mask_t;
     a.mask_r = ws.mask_r;
+    a.absmax_t = ws.absmax_part_t;
+    a.target_peak = ws.target_peak;
     a.levels.sumsq_t = ws.sumsq_part_t;
     a.levels.sumsq_r = ws.sumsq_part_r;
     a.levels.absmax_r = ws.absmax_part_r;

@@ -19,6 +19,7 @@ struct Workspace {
     float2* h_side;         // [2F+1]
     float* loud_values;     // [Dt][loud_capacity] counted mid samples of the convolution result with |mid| >= kLoudMid, per piece
     const float2** result_slot;  // device address of the convolution's result, recorded by the convolution kernel
+    float* target_peak;     // max|target|, written by spectrum_mean_kernel: the convolution's choice of precision needs it
     float2* conv_scratch;   // fft_size 16384 only: one padded 2F-point frame per CTA of convolve_global_kernel
     // ---- zeroed at the start of every job (one memset) ----
     unsigned char* zero_begin;

@@ -493,6 +493,7 @@ def check_edge_variant(variant, device):
     assert P % 2 == 1 and T % 2 == 1 and T % info["OUT"] != 0 and T > 5 * P
     ovs = variant.expected_ovs(P)
     assert ovs == variant.ovs, (variant.name, ovs)
+    assert run["state"].conv_precise == 0  # the float32 kernel under test did the work (convolve.cu: conv_precise)
     report = {}
     facts = check_pipeline(run, cfg, t, r, report, expect_ovs=ovs)
     # edges reached: several slots per piece with frames_per_piece not a multiple of them (where the geometry
