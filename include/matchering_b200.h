@@ -162,7 +162,10 @@ const char* mgb_last_error_string(void);
  * "analyze_chain": the analysis FFT builds twiddle powers in registers (1, default) or reads them all (0).  "design_direct": mgb_test_design_fir runs the
  * spline/LOWESS chain directly even when the plan has a smoothing operator.  "lookback_inclusive":
  * 0 makes limiter chunks publish aggregates only, so every look-back walks to its cut-off.  "limiter_ticket":
- * 1 hands the limiter's chunks out by an atomic ticket instead of the block index (0, default).
+ * 1 hands the limiter's chunks out by an atomic ticket instead of the block index (0, default).  "poison_alloc"
+ * (tests): 1 makes mgb_pipeline_create fill every device buffer it allocates with 0xFF bytes (NaN as a float or
+ * double, -1 as an integer), so that a read of slot memory no kernel wrote shows up in the results; 0 (default)
+ * leaves them as cudaMalloc returns them.
  * Returns MGB_ERR_INVALID for an unknown name. */
 int mgb_set_option(const char* name, int value);
 
@@ -380,7 +383,8 @@ int mgb_test_design_fir(const mgb_plan* plan, const double* d_avg, double* d_fir
                         void* stream);
 /* where the stages leave their hand-off values in a job's workspace: out[0..12] = byte offsets from d_workspace of
  * spec_part_t, spec_part_r, sumsq_part_t, sumsq_part_r, absmax_part_t, absmax_part_r, mask_t, mask_r, h_mid, h_side,
- * loud_values, piece_sums, loud_count; out[13] = loud_capacity (entries per piece); out[14..15] = 0. */
+ * loud_values, piece_sums, loud_count; out[13] = loud_capacity (entries per piece); out[14] = byte offset and out[15] =
+ * size of the limiter's tickets and look-back words (cleared by mgb_finalize before every limiter launch). */
 int mgb_test_workspace_regions(const mgb_plan* plan, const mgb_track_layout* layout, int64_t out[16]);
 
 #ifdef __cplusplus

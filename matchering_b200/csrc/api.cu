@@ -19,6 +19,7 @@ int g_conv_fused = 1;
 int g_conv_ovs = 4;
 int g_lookback_inclusive = 1;
 int g_limiter_ticket = 0;
+int g_poison_alloc = 0;
 
 #ifndef MGB_EMULATE
 long long g_launch_count = 0;
@@ -322,6 +323,10 @@ int mgb_set_option(const char* name, int value) {
     }
     if (strcmp(name, "design_direct") == 0) {
         g_design_direct = value ? 1 : 0;
+        return MGB_OK;
+    }
+    if (strcmp(name, "poison_alloc") == 0) {
+        g_poison_alloc = value ? 1 : 0;
         return MGB_OK;
     }
     if (host_set_option(name, value)) return MGB_OK;
@@ -730,6 +735,8 @@ int mgb_test_workspace_regions(const mgb_plan* plan, const mgb_track_layout* lay
     for (int i = 0; i < 16; ++i) out[i] = 0;
     for (int i = 0; i < 13; ++i) out[i] = (int64_t)reinterpret_cast<uintptr_t>(regions[i]);
     out[13] = w.loud_capacity;
+    out[14] = (int64_t)reinterpret_cast<uintptr_t>(w.tickets);  // the limiter's tickets and look-back words, which
+    out[15] = w.limiter_zero_bytes;                              // mgb_finalize clears before every limiter launch
     return MGB_OK;
 }
 

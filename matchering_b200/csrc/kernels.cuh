@@ -154,5 +154,6 @@ extern int g_conv_fused;     // convolution: ends of both transforms in register
 extern int g_conv_persistent;  // convolution (16384-point frames): one CTA per SM walks its frames, next frame's bulk copy under the epilogue
 extern int g_analyze_chain;  // analysis FFT: twiddle powers built in registers (1) or all read from the table (0)
 extern int g_twiddle_chain;  // convolution FFTs: build twiddle powers in registers (1) or read them all (0)
+extern int g_poison_alloc;   // tests: mgb_pipeline_create fills its device buffers with 0xFF bytes (1) or leaves them as allocated (0)
 
 }  // namespace mgb

@@ -68,9 +68,16 @@ struct SubmitGuard {
 };
 }  // namespace
 
+// With the "poison_alloc" option every new buffer starts as 0xFF bytes (NaN as float or double, -1 as an
+// integer), so that a kernel reading slot memory nothing wrote shows up in the results.
 #ifdef MGB_EMULATE
 #define MGB_CUDA_OK(call) (void)0
-static void* dev_alloc(size_t bytes) { return aligned_alloc(256, (bytes + 255) / 256 * 256); }
+static void* dev_alloc(size_t bytes) {
+    const size_t padded = (bytes + 255) / 256 * 256;
+    void* p = aligned_alloc(256, padded);
+    if (p && g_poison_alloc) memset(p, 0xFF, padded);
+    return p;
+}
 static void dev_free(void* p) { free(p); }
 #else
 #define MGB_CUDA_OK(call)                                                             \
@@ -83,7 +90,14 @@ static void dev_free(void* p) { free(p); }
     } while (0)
 static void* dev_alloc(size_t bytes) {
     void* p = nullptr;
-    return cudaMalloc(&p, bytes) == cudaSuccess ? p : nullptr;
+    if (cudaMalloc(&p, bytes) != cudaSuccess) return nullptr;
+    // (cudaMemset runs on the legacy default stream, which the pipeline's non-blocking streams do not wait for:
+    // the fill must be complete before the first submit's copies and kernels touch the buffer)
+    if (g_poison_alloc && (cudaMemset(p, 0xFF, bytes) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess)) {
+        cudaFree(p);
+        return nullptr;
+    }
+    return p;
 }
 static void dev_free(void* p) { cudaFree(p); }
 #endif
