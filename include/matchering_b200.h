@@ -51,7 +51,10 @@ typedef struct mgb_limiter_params {
     double threshold;   /* Config.threshold */
     int32_t reach;      /* make_odd(attack_samples) - 1 : half width of the centred max */
     int32_t hold;       /* hold_samples : length of the trailing max */
-    int32_t warmup;     /* samples after which attack_c^n < 1e-10 (halo of the attack filter) */
+    int32_t warmup;     /* samples after which attack_c^n < 1e-8: the halo kernel's warm-up of the attack filter.  Where
+                           warm-up, centred max and hold do not fit that kernel's span (8192 samples around a chunk),
+                           the library runs its wide-window path, which carries every window and filter state
+                           across chunks instead and needs more workspace (mgb_limiter_workspace_bytes) */
     int32_t hold_order;    /* LimiterConfig.hold_filter_order    (defaults.py:48-50) */
     int32_t release_order; /* LimiterConfig.release_filter_order (defaults.py:54-56) */
     int32_t reserved;
@@ -374,7 +377,8 @@ int mgb_test_fft(int32_t n, int32_t is_f64, int32_t dir, const void* d_in, void*
                  const void* d_twiddles, void* stream);
 /* the limiter's two scanned gain envelopes instead of its output: d_gains_out[n] = (attack gain g_att[n]
  * (hyrax.py:48-51, the filtfilt result), release gain max(hold_out, release_out)[n] (hyrax.py:56-75)).  Same
- * arguments as mgb_limit; kernels exist for the 44.1 / 96 kHz default windows. */
+ * arguments as mgb_limit; served on the halo kernel for the 44.1 / 96 kHz default windows, and for every Config that
+ * takes the wide-window path (windows wider than the halo kernel's span). */
 int mgb_test_limiter_gains(const mgb_limiter_params* params, const float* d_in_lr, float* d_gains_out, int64_t frames,
                            void* d_workspace, int64_t workspace_bytes, int32_t* d_engaged, void* stream);
 /* the FIR design alone from given average spectra: d_avg = [4][n_lin] doubles

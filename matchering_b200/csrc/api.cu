@@ -120,6 +120,7 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     w.tickets = (int*)take(256);
     w.lookback = take(limiter_lookback_bytes(plan.limiter, L.target_frames));
     w.limiter_zero_bytes = off - limiter_zero_from;
+    w.limiter_planes = take(limiter_plane_bytes(plan.limiter, L.target_frames));  // (empty unless the wide-window path runs)
     w.total_bytes = off;
     return w;
 }
@@ -559,18 +560,19 @@ int mgb_finalize(const mgb_plan* plan, const mgb_track_layout* L, const float* d
 #endif
         MGB_TRY(launch_limiter(plan->limiter, res, (float2*)d_out_limited, L->target_frames, &d_state->gain,
                                &d_state->final_amplitude_coef, &d_state->limiter_engaged, ws.tickets,
-                               ws.lookback, plan->d_limiter_tables, st));
+                               ws.lookback, ws.limiter_planes, plan->d_limiter_tables, st));
     }
     return MGB_OK;
 }
 
-// standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [256, kLimitHeader): pole tables  [kLimitHeader, ...): look-back words
+// standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [256, kLimitHeader): pole tables  [kLimitHeader, ...): look-back words,
+// then the wide-window path's planes (none for the halo kernel)
 static const int64_t kLimitHeader = 256 + 32768;
 
 int64_t mgb_limiter_workspace_bytes(const mgb_limiter_params* params, int64_t frames) {
     if (!params) return -1;
     if (frames <= 0) return kLimitHeader;
-    return kLimitHeader + limiter_lookback_bytes(*params, frames);
+    return kLimitHeader + limiter_lookback_bytes(*params, frames) + limiter_plane_bytes(*params, frames);
 }
 
 static int limit_impl(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,
@@ -600,7 +602,7 @@ static int limit_impl(const mgb_limiter_params* params, const float* d_in_lr, fl
     MGB_TRY(launch_absmax((const float2*)d_in_lr, frames, peak, st));
     MGB_TRY(launch_limiter_engaged(peak, nullptr, params->threshold, d_engaged, st));
     return launch_limiter(*params, (const float2*)d_in_lr, (float2*)d_out_lr, frames, nullptr, nullptr, d_engaged, ticket,
-                          base + kLimitHeader, tables, st, gains_only);
+                          base + kLimitHeader, base + zero_bytes, tables, st, gains_only);
 }
 
 int mgb_limit(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,

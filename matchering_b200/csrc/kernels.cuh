@@ -31,6 +31,7 @@ struct Workspace {
     int* tickets;           // [64] zeroed counters: 0 = limiter chunk ticket
     unsigned char* lookback;// [nchunks] LookbackSlot
     int64_t limiter_zero_bytes;
+    unsigned char* limiter_planes;  // the wide-window limiter's planes (limiter_plane_bytes; none for the halo kernel)
     int64_t design_stride;  // doubles per channel in `design`
     int64_t total_bytes;
 };
@@ -129,9 +130,20 @@ int launch_convert_f64_f32(const double* in, float* out, int64_t count, cudaStre
 int launch_convert_f32_f64(const float* in, double* out, int64_t count, cudaStream_t stream);
 
 // limiter.cu ------------------------------------------------------------------------------------
+// (the halo kernel where its span fits, the wide-window path otherwise; wide_planes: limiter_plane_bytes of workspace)
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
-                   const double* post_gain, const int* engaged, int* ticket, void* lookback, const void* tables,
-                   cudaStream_t stream, bool gains_only = false);
+                   const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
+                   const void* tables, cudaStream_t stream, bool gains_only = false);
+int limiter_validate(const mgb_limiter_params& lp);
+bool limiter_span_too_wide(const mgb_limiter_params& lp);  // the wide-window path serves these parameters
+int64_t limiter_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // its workspace planes; 0 for the halo kernel
+
+// limiter_wide.cuh --------------------------------------------------------------------------------
+int64_t limiter_wide_lookback_bytes(const mgb_limiter_params& lp, int64_t frames, int order_capacity);
+int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames);
+int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
+                        int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
+                        void* planes, const void* tables, cudaStream_t stream, bool gains_only);
 int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream_t stream);
 int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, double threshold, int* engaged,
                            cudaStream_t stream);

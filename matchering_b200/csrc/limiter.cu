@@ -25,15 +25,13 @@
 #include <math.h>
 #include <string.h>
 
-#include "kernels.cuh"
+#include "limiter_scan.cuh"
+#include "limiter_wide.cuh"  // the wide-window path: windows wider than this kernel's span
 
 namespace mgb {
 
 namespace {
 
-constexpr int NT = kLimiterThreads;
-constexpr int CORE_EPT = kLimiterCoreEpt;
-constexpr int LC = kLimiterCore;
 constexpr int SPAN_EPT_MAX = kLimiterSpanEptMax;
 
 // Exclusive carry of the recurrence y = u + p*y_prev across the block: given each thread's local
@@ -92,224 +90,6 @@ __device__ __forceinline__ double scan_carry_rev(double B, const ScanPow* t, con
     double prev = __shfl_down_sync(0xffffffffu, v, 1);
     if (rl == 0) prev = 0.0;
     return prev + t->ql[rl] * ((rw > 0 ? warp_carry : 0.0) + t->qw[rw] * (*c0));
-}
-
-// ------------------------------------------------------------------------------------------------
-// Recursive sections of order N (hold and release low-passes).  lfilter(b, a, x) is
-//     y[n] = sum_{i=0..N} b[i] x[n-i] - sum_{i=1..N} a[i] y[n-i]          (a[0] = 1, zero initial state)
-// The feed-forward sum is formed per sample from the thread's own inputs; the recursion is a linear
-// recurrence over the STATE s = (y[n-1], ..., y[n-N]) with the companion matrix C (row 0 = -a[1..N], row i =
-// e_{i-1}): a segment maps s -> C^len s + (its zero-state end state), which is what the blocked scan and the
-// look-back combine.  N = 1 is the scalar scan of a single pole; every loop below unrolls away there.
-// ------------------------------------------------------------------------------------------------
-template <int N>
-struct StVec {
-    double v[N];
-};
-template <int N>
-__device__ __forceinline__ StVec<N> st_zero() {
-    StVec<N> z;
-#pragma unroll
-    for (int i = 0; i < N; ++i) z.v[i] = 0.0;
-    return z;
-}
-template <int N>
-__device__ __forceinline__ StVec<N> st_shfl_up(StVec<N> a, int d) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) a.v[i] = __shfl_up_sync(0xffffffffu, a.v[i], d);
-    return a;
-}
-template <int N>
-__device__ __forceinline__ StVec<N> st_shfl(StVec<N> a, int src) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) a.v[i] = __shfl_sync(0xffffffffu, a.v[i], src);
-    return a;
-}
-// y += M x
-template <int N>
-__device__ __forceinline__ void st_addmul(StVec<N>& y, const double (*M)[N], const StVec<N>& x) {
-#pragma unroll
-    for (int r = 0; r < N; ++r)
-#pragma unroll
-        for (int c = 0; c < N; ++c) y.v[r] += M[r][c] * x.v[c];
-}
-template <int N>
-__device__ __forceinline__ StVec<N> st_mul(const double (*M)[N], const StVec<N>& x) {
-    StVec<N> y = st_zero<N>();
-    st_addmul<N>(y, M, x);
-    return y;
-}
-
-// Exclusive carry of the section's state across the block: given each thread's zero-state end state B, returns
-// the state just before the thread's first element when the state before the block's first element is zero
-// (the chunk's carry-in is added later, section_lead).  Same structure and the same single barrier as
-// scan_carry; scratch: >= 32*N doubles, alternate between two buffers.  Every thread of the block must call.
-template <int N>
-__device__ __forceinline__ StVec<N> section_scan(StVec<N> B, const SectionTab<N>* t, double* scratch) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    StVec<N> v = B;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const StVec<N> up = st_shfl_up<N>(v, d);
-        if (lane >= d) st_addmul<N>(v, t->ql[d], up);
-    }
-    if (lane == 31) {
-#pragma unroll
-        for (int i = 0; i < N; ++i) scratch[warp * N + i] = v.v[i];
-    }
-    __syncthreads();
-    StVec<N> w = st_zero<N>();
-    if (lane < NT / 32) {
-#pragma unroll
-        for (int i = 0; i < N; ++i) w.v[i] = scratch[lane * N + i];
-    }
-#pragma unroll
-    for (int d = 1; d < NT / 32; d <<= 1) {
-        const StVec<N> up = st_shfl_up<N>(w, d);
-        if (lane >= d) st_addmul<N>(w, t->qw[d], up);
-    }
-    // state at the end of the previous warp: inclusive total of warps 0..warp-1
-    StVec<N> warp_carry = st_shfl<N>(w, (warp + 31) & 31);
-    if (warp == 0) warp_carry = st_zero<N>();
-    StVec<N> prev = st_shfl_up<N>(v, 1);
-    if (lane == 0) prev = st_zero<N>();
-    st_addmul<N>(prev, t->ql[lane], warp_carry);
-    return prev;
-}
-
-// C^(tid * CORE_EPT) applied to the chunk's carry-in: what the carry-in contributes to the state just before
-// the thread's first element.
-template <int N>
-__device__ __forceinline__ StVec<N> section_lead(const SectionTab<N>* t, const StVec<N>& cin) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    return st_mul<N>(t->ql[lane], st_mul<N>(t->qw[warp], cin));
-}
-
-// 16-byte publish / poll of a LookbackWord through L2 (st.cg / ld.cg: coherent device-wide).
-__device__ __forceinline__ void publish(LookbackWord* w, double v, int status) {
-#ifdef MGB_EMULATE
-    w->value = v;
-    w->status = status;
-#else
-    asm volatile("st.global.cg.v2.u64 [%0], {%1, %2};" ::"l"(w), "l"(__double_as_longlong(v)), "l"((long long)status) : "memory");
-#endif
-}
-__device__ __forceinline__ int poll(const LookbackWord* w, double* v) {
-#ifdef MGB_EMULATE
-    *v = w->value;
-    return (int)w->status;
-#else
-    long long a, b;
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(w) : "memory");
-    *v = __longlong_as_double(a);
-    return (int)b;
-#endif
-}
-
-// Carry into chunk `chunk` of a section whose per-chunk transition is P = pc[1] (decoupled look-back).  One warp
-// inspects 32 predecessors at a time: every lane polls one predecessor's words, the window is cut at the nearest
-// predecessor whose INCLUSIVE state is known, each lane weighs its state by P^distance, and one warp reduction
-// at the very end adds them up.  The walk stops when whatever lies further back weighs less than 1e-9 (all
-// states are gains in [0, 1], so that bounds the absolute error of the carry).  A state of N doubles travels as
-// N words that each carry the status: a reader that catches the writer between two words sees different
-// statuses and polls again.  Called by all 32 lanes of one warp.
-template <int N>
-__device__ __forceinline__ StVec<N> lookback(const LookbackWord* words /* this section's words of chunk 0 */, int chunk,
-                                             const SectionTab<N>* t) {
-    constexpr int STRIDE = 2 * N;  // words per chunk: hold[N] then release[N]
-    const int lane = threadIdx.x & 31;
-    if constexpr (N == 1) {
-        // a single pole: scalar weights, the running product P^32, P^64, ... is exact enough (no table)
-        double acc1 = 0.0, m1 = 1.0;
-        for (int base = chunk - 1; base >= 0 && m1 > 1e-9; base -= 32) {
-            const int j = base - lane;
-            int st = 2;  // before the first chunk: inclusive state 0 (lfilter starts from rest)
-            double val = 0.0;
-            if (j >= 0) {
-                const LookbackWord* w = words + (long long)j * STRIDE;
-                while ((st = poll(w, &val)) == 0) __nanosleep(20);
-            }
-            const unsigned inclusive = __ballot_sync(0xffffffffu, st == 2);
-            const int first = inclusive ? __ffs((int)inclusive) - 1 : 32;
-            if (lane <= first) acc1 += m1 * t->pc[lane][0][0] * val;
-            if (inclusive) break;
-            m1 *= t->pc[32][0][0];
-        }
-        StVec<N> out;
-        out.v[0] = warp_sum(acc1);
-        return out;
-    }
-    StVec<N> acc = st_zero<N>();
-    double mult[N][N];  // C^(LC*32*jump): weight of this window's nearest chunk
-    int jump = 0;       // windows of 32 chunks already behind us
-    for (int base = chunk - 1; base >= 0; base -= 32, ++jump) {
-        // From the table (a running product would cost a digit per multiplication for a pole pair); beyond
-        // the table -- 2048 chunks back, where the weights of any ordinary release are long below the cut-off
-        // -- the product of what is left is good enough.
-        if (N > 1 && jump < kLookbackJumps) {
-#pragma unroll
-            for (int r = 0; r < N; ++r)
-#pragma unroll
-                for (int c = 0; c < N; ++c) mult[r][c] = t->pj[jump][r][c];
-        } else if (jump == 0) {
-#pragma unroll
-            for (int r = 0; r < N; ++r)
-#pragma unroll
-                for (int c = 0; c < N; ++c) mult[r][c] = r == c ? 1.0 : 0.0;
-        } else {  // (a single pole: the running product is exact enough, no table)
-            double next[N][N];
-#pragma unroll
-            for (int r = 0; r < N; ++r)
-#pragma unroll
-                for (int c = 0; c < N; ++c) {
-                    double sum = 0.0;
-#pragma unroll
-                    for (int k = 0; k < N; ++k) sum += mult[r][k] * t->pc[32][k][c];
-                    next[r][c] = sum;
-                }
-#pragma unroll
-            for (int r = 0; r < N; ++r)
-#pragma unroll
-                for (int c = 0; c < N; ++c) mult[r][c] = next[r][c];
-        }
-        // (past its peak at 1/(1-|p|) samples the norm of C^m only falls: once this window's nearest chunk
-        // weighs less than 1e-9, so does everything behind it)
-        double bound = 0.0;
-#pragma unroll
-        for (int r = 0; r < N; ++r) {
-            double rowsum = 0.0;
-#pragma unroll
-            for (int c = 0; c < N; ++c) rowsum += fabs(mult[r][c]);
-            bound = fmax(bound, rowsum);
-        }
-        if (bound <= 1e-9) break;
-        const int j = base - lane;
-        int st = 2;  // before the first chunk: inclusive state 0 (lfilter starts from rest)
-        StVec<N> val = st_zero<N>();
-        if (j >= 0) {
-            const LookbackWord* w = words + (long long)j * STRIDE;
-            for (;;) {
-                st = poll(w, &val.v[0]);
-                bool same = st != 0;
-#pragma unroll
-                for (int i = 1; i < N; ++i) same = same && poll(w + i, &val.v[i]) == st;
-                if (same) break;
-                __nanosleep(20);
-            }
-        }
-        const unsigned inclusive = __ballot_sync(0xffffffffu, st == 2);
-        const int first = inclusive ? __ffs((int)inclusive) - 1 : 32;
-        if (lane <= first) st_addmul<N>(acc, mult, st_mul<N>(t->pc[lane], val));
-        if (inclusive) break;
-    }
-#pragma unroll
-    for (int i = 0; i < N; ++i) acc.v[i] = warp_sum(acc.v[i]);
-    return acc;
-}
-template <int N>
-__device__ __forceinline__ void publish_state(LookbackWord* words, const StVec<N>& s, int status) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) publish(words + i, s.v[i], status);
 }
 
 struct LimiterGeom {
@@ -787,15 +567,34 @@ int limiter_order_capacity(const mgb_limiter_params& lp) {
     return (lp.hold_order <= 1 && lp.release_order <= 1) ? 1 : MGB_MAX_FILTER_ORDER;
 }
 
-int limiter_geometry(const mgb_limiter_params& lp, LimiterGeom* g) {
+}  // namespace
+
+int limiter_validate(const mgb_limiter_params& lp) {
     MGB_REQUIRE(lp.reach >= 1 && lp.hold >= 3 && lp.warmup >= 8, MGB_ERR_INVALID, "limiter: bad window sizes");
     MGB_REQUIRE(lp.hold_order >= 1 && lp.hold_order <= MGB_MAX_FILTER_ORDER && lp.release_order >= 1 &&
                     lp.release_order <= MGB_MAX_FILTER_ORDER,
                 MGB_ERR_UNSUPPORTED, "limiter: hold / release filter orders %d / %d, kernels exist for 1..%d", lp.hold_order,
                 lp.release_order, MGB_MAX_FILTER_ORDER);
-    const int no = limiter_order_capacity(lp);
     MGB_REQUIRE(lp.attack_c > 0.0 && lp.attack_c < 1.0, MGB_ERR_INVALID, "limiter: attack pole out of (0,1)");
     MGB_REQUIRE(lp.threshold > 0.0, MGB_ERR_INVALID, "limiter: threshold must be positive");
+    return MGB_OK;
+}
+
+// The halo kernel serves the parameters exactly when its span fits (limiter_geometry: ept <= kLimiterSpanEptMax);
+// the wide-window path (limiter_wide.cuh) serves all others.  The span in 64 bits: a slow attack's warm-up
+// overflows int.  (Rounding ept up to odd, or to its minimum of 11, never crosses 25.)
+bool limiter_span_too_wide(const mgb_limiter_params& lp) {
+    const long long no = limiter_order_capacity(lp), warm = lp.warmup, hold = lp.hold, reach = lp.reach;
+    const long long left = warm > hold + no - 1 ? warm : hold + no - 1;
+    const long long span = LC + left + warm + 2 * reach;
+    return (span + NT - 1) / NT > SPAN_EPT_MAX;
+}
+
+namespace {
+
+int limiter_geometry(const mgb_limiter_params& lp, LimiterGeom* g) {
+    MGB_TRY(limiter_validate(lp));
+    const int no = limiter_order_capacity(lp);
     g->reach = lp.reach;
     g->hold = lp.hold;
     g->warm = lp.warmup;
@@ -906,14 +705,22 @@ int64_t limiter_lookback_bytes(int64_t frames, int order_capacity) {
     return (chunks * 2 * order_capacity * (int64_t)sizeof(LookbackWord) + 255) / 256 * 256;
 }
 int64_t limiter_lookback_bytes(const mgb_limiter_params& lp, int64_t frames) {
+    if (limiter_span_too_wide(lp)) return limiter_wide_lookback_bytes(lp, frames, limiter_order_capacity(lp));
     return limiter_lookback_bytes(frames, limiter_order_capacity(lp));
+}
+int64_t limiter_plane_bytes(const mgb_limiter_params& lp, int64_t frames) {
+    return limiter_span_too_wide(lp) ? limiter_wide_plane_bytes(lp, frames) : 0;
 }
 
 int64_t limiter_tables_bytes() { return (int64_t)(sizeof(ScanPow) + 2 * sizeof(SectionTab<MGB_MAX_FILTER_ORDER>) + 255) / 256 * 256; }
 
 int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream_t stream) {
     LimiterGeom g;
-    MGB_TRY(limiter_geometry(lp, &g));
+    MGB_TRY(limiter_validate(lp));
+    if (limiter_span_too_wide(lp))
+        g.ept = CORE_EPT;  // the wide-window path scans the attack filter over CORE_EPT samples per thread
+    else
+        MGB_TRY(limiter_geometry(lp, &g));
     if (limiter_order_capacity(lp) == 1)
         return launch("limiter_tables_kernel", limiter_tables_kernel, dim3(1), dim3(64), 0, stream, lp, g.ept,
                       (unsigned char*)tables);
@@ -937,12 +744,16 @@ int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream
 }
 
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
-                   const double* post_gain, const int* engaged, int* ticket, void* lookback, const void* tables,
-                   cudaStream_t stream, bool gains_only) {
-    LimiterGeom g;
-    MGB_TRY(limiter_geometry(lp, &g));
+                   const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
+                   const void* tables, cudaStream_t stream, bool gains_only) {
+    MGB_TRY(limiter_validate(lp));
     MGB_REQUIRE(frames > 6, MGB_ERR_INVALID, "limiter: the input must be longer than filtfilt's padlen (6)");
     MGB_REQUIRE(tables != nullptr, MGB_ERR_INVALID, "limiter: pole tables missing");
+    if (limiter_span_too_wide(lp))  // (chunks by block index: the wide-window path has no ticket)
+        return launch_limiter_wide(lp, limiter_order_capacity(lp), g_lookback_inclusive, in, out, frames, pre_gain, post_gain,
+                                   engaged, lookback, wide_planes, tables, stream, gains_only);
+    LimiterGeom g;
+    MGB_TRY(limiter_geometry(lp, &g));
     const int64_t chunks = (frames + LC - 1) / LC;
     const size_t smem = (size_t)g.ept * NT * 16 + (size_t)g.margin * 8;
     const int no = limiter_order_capacity(lp);

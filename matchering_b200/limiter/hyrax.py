@@ -52,11 +52,12 @@ def _limit_host(array: np.ndarray, params, device, lib):
         raise ValueError("The length of the input vector x must be greater than padlen, which is 6.")
     io = HostIO.get()
     with torch.cuda.device(device):
-        key = (device.index, frames, params.hold_order, params.release_order)  # (the workspace depends on the orders)
+        # (the workspace depends on the orders and, on the wide-window path, on the windows: key on its size)
+        ws_bytes = int(lib.mgb_limiter_workspace_bytes(C.byref(params), frames))
+        key = (device.index, frames, ws_bytes)
         bufs = _LIMIT_BUFFERS.get(key)
         if bufs is None:
             _LIMIT_BUFFERS.clear()  # one size cached: an hour of audio is 1.3 GB per buffer
-            ws_bytes = int(lib.mgb_limiter_workspace_bytes(C.byref(params), frames))
             bufs = _LIMIT_BUFFERS[key] = dict(
                 x=torch.empty((frames, 2), dtype=torch.float32, device=device),
                 y=torch.empty((frames, 2), dtype=torch.float32, device=device),

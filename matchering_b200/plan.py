@@ -212,7 +212,6 @@ class LimiterConstants:
 
 
 MAX_FILTER_ORDER = 2   # MGB_MAX_FILTER_ORDER
-MAX_LIMITER_HALO = 8192  # left + right halo the limiter kernel's shared-memory span can hold (kLimiterSpanEptMax = 25)
 
 
 def limiter_constants(config) -> LimiterConstants:
@@ -235,9 +234,7 @@ def limiter_constants(config) -> LimiterConstants:
     if not 0.0 < c < 1.0:
         raise UnsupportedConfig("attack_filter_coefficient must be negative (a decaying one-pole)")
     warmup = int(math.ceil(math.log(1e-8) / math.log(c)))
-    warmup = max(32, (warmup + 31) // 32 * 32)
-    if 2 * warmup + hold + 2 * reach + 64 > MAX_LIMITER_HALO:
-        raise UnsupportedConfig("attack filter decays too slowly for the limiter kernel's halo")
+    warmup = max(32, (warmup + 31) // 32 * 32)  # (the halo kernel's warm-up; wider windows take the wide-window path)
     bh, ah = _signal.butter(lim.hold_filter_order, lim.hold_filter_coefficient, fs=sr)
     br, ar = _signal.butter(lim.release_filter_order, lim.release_filter_coefficient / lim.release, fs=sr)
     return LimiterConstants(config.threshold, reach, hold, warmup, c, bh, ah, br, ar)
