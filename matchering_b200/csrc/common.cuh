@@ -207,16 +207,17 @@ __device__ __forceinline__ void atomic_max_nonneg(float* addr, float v) {
 // the barrier's phase parity.  Sizes and both addresses must be multiples of 16 bytes.
 // ------------------------------------------------------------------------------------------------
 #ifdef MGB_EMULATE
+// the completed phase is a release by the copying thread and an acquire by each waiter, as the mbarrier's is
 struct TmaBarrier {
-    volatile unsigned phase_done;  // number of completed phases
+    unsigned phase_done;  // number of completed phases
 };
-__device__ __forceinline__ void tma_barrier_init(TmaBarrier* b) { b->phase_done = 0; }
+__device__ __forceinline__ void tma_barrier_init(TmaBarrier* b) { __atomic_store_n(&b->phase_done, 0u, __ATOMIC_RELAXED); }
 __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, TmaBarrier* b) {
     if (bytes) memcpy(smem_dst, gmem_src, bytes);
-    b->phase_done = b->phase_done + 1;
+    __atomic_fetch_add(&b->phase_done, 1u, __ATOMIC_RELEASE);
 }
 __device__ __forceinline__ void tma_barrier_wait(TmaBarrier* b, uint32_t phase_index) {
-    while (b->phase_done <= phase_index) ::emul::yield();
+    while (__atomic_load_n(&b->phase_done, __ATOMIC_ACQUIRE) <= phase_index) ::emul::yield();
 }
 __device__ __forceinline__ void fence_proxy_async() {}
 #else

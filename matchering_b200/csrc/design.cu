@@ -188,22 +188,21 @@ __device__ double block_kth_smallest(const double* __restrict__ v, int n, int k)
     __shared__ unsigned long long sel_prefix;
     __shared__ int sel_rank;
     const int tid = threadIdx.x, nthr = blockDim.x;
-    if (tid == 0) {
-        sel_prefix = 0ull;
-        sel_rank = k;
-    }
+    // The first pass starts from prefix 0 and rank k without reading sel_prefix / sel_rank: other threads may
+    // still be reading the previous call's result there.  Thread 0 first writes them after this call's
+    // second barrier, which every thread reaches only after that read.
     unsigned long long mask = 0ull;
     for (int shift = 56; shift >= 0; shift -= 8) {
         for (int b = tid; b < 256; b += nthr) hist[b] = 0u;
         __syncthreads();
-        const unsigned long long prefix = sel_prefix;
+        const unsigned long long prefix = shift == 56 ? 0ull : sel_prefix;
         for (int j = tid; j < n; j += nthr) {
             const unsigned long long bits = (unsigned long long)__double_as_longlong(v[j]);
             if ((bits & mask) == prefix) atomicAdd(&hist[(unsigned)(bits >> shift) & 255u], 1u);
         }
         __syncthreads();
         if (tid == 0) {
-            int rank = sel_rank, b = 0;
+            int rank = shift == 56 ? k : sel_rank, b = 0;
             while (b < 255 && rank >= (int)hist[b]) {
                 rank -= (int)hist[b];
                 ++b;
@@ -278,7 +277,7 @@ __device__ void smooth_curve(const mgb_plan& plan, double* __restrict__ base) {
             acc_b = warp_sum(acc_b);
             if (lane == 0) {
                 zz[f] = acc_a;
-                zz[f2] = acc_b;
+                if (f + nwarps < nfit) zz[f2] = acc_b;  // else f2 is clamped: nfit - 1 is another warp's
             }
         }
         __syncthreads();

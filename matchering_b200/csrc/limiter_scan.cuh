@@ -105,16 +105,17 @@ __device__ __forceinline__ StVec<N> section_lead(const SectionTab<N>* t, const S
 // 16-byte publish / poll of a LookbackWord through L2 (st.cg / ld.cg: coherent device-wide).
 __device__ __forceinline__ void publish(LookbackWord* w, double v, int status) {
 #ifdef MGB_EMULATE
-    w->value = v;
-    w->status = status;
+    // value and status travel together in one 16-byte store: two 8-byte atomics are as close as the host gets
+    __atomic_store_n((long long*)&w->value, __double_as_longlong(v), __ATOMIC_RELAXED);
+    __atomic_store_n(&w->status, (long long)status, __ATOMIC_RELAXED);
 #else
     asm volatile("st.global.cg.v2.u64 [%0], {%1, %2};" ::"l"(w), "l"(__double_as_longlong(v)), "l"((long long)status) : "memory");
 #endif
 }
 __device__ __forceinline__ int poll(const LookbackWord* w, double* v) {
 #ifdef MGB_EMULATE
-    *v = w->value;
-    return (int)w->status;
+    *v = __longlong_as_double(__atomic_load_n((const long long*)&w->value, __ATOMIC_RELAXED));
+    return (int)__atomic_load_n(&w->status, __ATOMIC_RELAXED);
 #else
     long long a, b;
     asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(w) : "memory");

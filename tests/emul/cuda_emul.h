@@ -8,6 +8,36 @@
 // kernels always find their predecessors finished.  It checks kernel LOGIC (indexing, barriers,
 // scan carries) against the oracle; it proves nothing about performance and is never loaded by
 // the product package (matchering_b200/_native.py only ever loads the nvcc-built library).
+//
+// Memory a block has not written is not trusted to be benign:
+// - Dynamic shared memory is a fresh allocation at every block start, filled with 0xFF (NaN as a
+//   float or double, -1 as an int), so a read of a word the block never wrote shows up in the result.
+// - Static `__shared__` arrays are thread_local statics: they keep the previous block's values.
+//
+// Schedule: between two synchronisation points a fiber runs alone, and each round resumes the
+// block's ready fibers in the order MGB_EMUL_ORDER names: `forward` (ascending thread index, the
+// default), `reverse`, or `seeded` (a fresh permutation every round from MGB_EMUL_SEED, default 1).
+// A missing barrier whose reader runs after its writer in one order runs before it in another.
+//
+// Race checking (-DMGB_EMUL_RACECHECK, with the kernel sources built -fsanitize=thread): every
+// emulated thread is a ThreadSanitizer fiber, created for its block and destroyed at the block's end,
+// and switches between fibers carry no happens-before edge.  Edges exist only where CUDA gives them:
+// - __syncthreads: release on arrival, acquire on departure (an exited thread counts as arrived);
+// - __syncwarp and the warp shuffles / votes: the same among the warp's participating lanes;
+// - atomics are relaxed __atomic operations: concurrent ones are not races, and they order nothing;
+// - TMA completion: release by the copying thread, acquire by each waiter;
+// - a launch is ordered after the host code before it, and the host code after it after the whole
+//   launch.  Blocks of one launch are also ordered one after another: races BETWEEN blocks are not
+//   looked for, since static `__shared__` arrays cannot be given fresh shadow memory per block.
+// - ThreadSanitizer tells at most 256 live threads apart.  A block of more than 224 threads therefore shares
+//   fibers among lanes of one warp, in one of two groupings that alternate by block and launch (cuda_emul.cpp);
+//   every pair of lanes has fibers of its own in one of them.  A kernel launched once with a single block is
+//   seen in one grouping only: there, races between the few lanes of a warp that share a fiber go unreported.
+// - A warp keeps one barrier counter, and a warp barrier completes when as many lanes as its mask names
+//   have arrived.  Two disjoint lane groups of one warp that synchronise under partial masks at the same time
+//   would be ordered with each other, which CUDA does not do.  (Every warp intrinsic in the kernels names the
+//   full warp.)
+// The scheduler and its bookkeeping live in cuda_emul.cpp, which is never instrumented.
 #pragma once
 #ifndef MGB_EMULATE
 #error "cuda_emul.h is only for -DMGB_EMULATE host builds"
@@ -65,12 +95,14 @@ struct Fiber {
     char* stack = nullptr;
     bool done = false;
     unsigned tid = 0;
+    void* tsan = nullptr;  // the fiber's ThreadSanitizer context (race-checking build)
 };
 
 struct WarpState {
     uint64_t vals[32];
     unsigned arrived = 0, gen = 0;
     unsigned ballot_acc = 0;
+    char sync[2];  // release/acquire objects of the warp barrier, by generation parity
 };
 
 struct BlockState {
@@ -80,14 +112,24 @@ struct BlockState {
     std::vector<WarpState> warps;
     std::function<void()> body;
     void* sched_sp = nullptr;
+    void* sched_tsan = nullptr;
     unsigned current = 0;
-    std::vector<unsigned char> dyn_smem;
+    unsigned char* dyn_smem = nullptr;
+    char sync[2];         // release/acquire objects of __syncthreads, by generation parity
+    char exit_sync;       // threads that have exited -> the arrival that completes a barrier
+    char start_sync, end_sync;  // host -> every fiber at its start; every fiber at its end -> host
 };
 
 BlockState& block();
 void yield();
 void launch(dim3 grid, dim3 blockdim, size_t smem_bytes, const std::function<void()>& body);
 unsigned char* dyn_smem();
+// The synchronisation points, in cuda_emul.cpp so that the race-checking build never instruments the
+// scheduler's bookkeeping: the block barrier, a barrier of `expected` lanes of the caller's warp, and a
+// shuffle of a raw 8-byte payload from `src_lane`.
+void syncthreads();
+void warp_barrier(unsigned expected);
+uint64_t shfl_raw(unsigned expected, uint64_t raw, unsigned src_lane);
 
 }  // namespace emul
 
@@ -97,29 +139,10 @@ extern thread_local dim3 blockDim;
 extern thread_local dim3 gridDim;
 
 // ----------------------------------------------------------------------------- barriers
-static inline void __syncthreads() {
-    emul::BlockState& b = emul::block();
-    unsigned gen = b.gen;
-    if (++b.arrived >= b.alive) {
-        b.arrived = 0;
-        b.gen++;
-    } else {
-        while (b.gen == gen) emul::yield();
-    }
-}
+static inline void __syncthreads() { emul::syncthreads(); }
 
 namespace emul {
-static inline void warp_barrier(WarpState& w, unsigned expected) {
-    unsigned gen = w.gen;
-    if (++w.arrived >= expected) {
-        w.arrived = 0;
-        w.gen++;
-    } else {
-        while (w.gen == gen) emul::yield();
-    }
-}
 static inline unsigned lane_id() { return threadIdx.x & 31u; }
-static inline WarpState& my_warp() { return block().warps[threadIdx.x >> 5]; }
 static inline unsigned warp_width() {
     // number of live lanes in this warp (last warp of a block may be partial)
     unsigned base = threadIdx.x & ~31u;
@@ -129,14 +152,10 @@ static inline unsigned warp_width() {
 template <typename T>
 static inline T shfl_generic(unsigned mask, T v, int src_lane) {
     static_assert(sizeof(T) <= 8, "shuffle payload");
-    WarpState& w = my_warp();
     unsigned expected = std::min<unsigned>(__builtin_popcount(mask), warp_width());
     uint64_t raw = 0;
     std::memcpy(&raw, &v, sizeof(T));
-    w.vals[lane_id()] = raw;
-    warp_barrier(w, expected);
-    uint64_t got = w.vals[(unsigned)src_lane & 31u];
-    warp_barrier(w, expected);
+    uint64_t got = shfl_raw(expected, raw, (unsigned)src_lane & 31u);
     T out;
     std::memcpy(&out, &got, sizeof(T));
     return out;
@@ -144,7 +163,7 @@ static inline T shfl_generic(unsigned mask, T v, int src_lane) {
 }  // namespace emul
 
 static inline void __syncwarp(unsigned mask = 0xffffffffu) {
-    emul::warp_barrier(emul::my_warp(), std::min<unsigned>(__builtin_popcount(mask), emul::warp_width()));
+    emul::warp_barrier(std::min<unsigned>(__builtin_popcount(mask), emul::warp_width()));
 }
 template <typename T>
 static inline T __shfl_sync(unsigned mask, T v, int src, int width = 32) {
@@ -200,17 +219,31 @@ static inline T __ldg(const T* p) { return *p; }
 template <typename T>
 static inline T __ldcg(const T* p) { return *(const volatile T*)p; }
 
-static inline int atomicAdd(int* p, int v) { int o = *p; *p = o + v; return o; }
-static inline unsigned atomicAdd(unsigned* p, unsigned v) { unsigned o = *p; *p = o + v; return o; }
-static inline unsigned long long atomicAdd(unsigned long long* p, unsigned long long v) { auto o = *p; *p = o + v; return o; }
-static inline float atomicAdd(float* p, float v) { float o = *p; *p = o + v; return o; }
-static inline double atomicAdd(double* p, double v) { double o = *p; *p = o + v; return o; }
-static inline int atomicMax(int* p, int v) { int o = *p; if (v > o) *p = v; return o; }
-static inline unsigned atomicMax(unsigned* p, unsigned v) { unsigned o = *p; if (v > o) *p = v; return o; }
-static inline int atomicExch(int* p, int v) { int o = *p; *p = v; return o; }
-static inline unsigned atomicExch(unsigned* p, unsigned v) { unsigned o = *p; *p = v; return o; }
-static inline int atomicCAS(int* p, int c, int v) { int o = *p; if (o == c) *p = v; return o; }
-static inline unsigned atomicOr(unsigned* p, unsigned v) { unsigned o = *p; *p = o | v; return o; }
+// Relaxed, like CUDA's atomics: concurrent ones are not a race, and none of them orders other accesses.
+namespace emul {
+template <typename T, typename F>
+static inline T atomic_rmw(T* p, F f) {
+    T o, n;
+    __atomic_load(p, &o, __ATOMIC_RELAXED);
+    do n = f(o);
+    while (!__atomic_compare_exchange(p, &o, &n, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED));
+    return o;
+}
+}  // namespace emul
+static inline int atomicAdd(int* p, int v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline unsigned atomicAdd(unsigned* p, unsigned v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline unsigned long long atomicAdd(unsigned long long* p, unsigned long long v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+static inline float atomicAdd(float* p, float v) { return emul::atomic_rmw(p, [v](float o) { return o + v; }); }
+static inline double atomicAdd(double* p, double v) { return emul::atomic_rmw(p, [v](double o) { return o + v; }); }
+static inline int atomicMax(int* p, int v) { return emul::atomic_rmw(p, [v](int o) { return v > o ? v : o; }); }
+static inline unsigned atomicMax(unsigned* p, unsigned v) { return emul::atomic_rmw(p, [v](unsigned o) { return v > o ? v : o; }); }
+static inline int atomicExch(int* p, int v) { return __atomic_exchange_n(p, v, __ATOMIC_RELAXED); }
+static inline unsigned atomicExch(unsigned* p, unsigned v) { return __atomic_exchange_n(p, v, __ATOMIC_RELAXED); }
+static inline int atomicCAS(int* p, int c, int v) {
+    __atomic_compare_exchange_n(p, &c, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED);
+    return c;
+}
+static inline unsigned atomicOr(unsigned* p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 
 // ----------------------------------------------------------------------------- math intrinsics
 static inline int __float_as_int(float f) { int i; std::memcpy(&i, &f, 4); return i; }

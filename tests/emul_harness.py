@@ -16,10 +16,13 @@ _LIB = None
 
 
 def emul_lib():
+    """The emulator library; with MGB_EMUL_BUILD=racecheck, its ThreadSanitizer build (which needs libtsan
+    preloaded into the process: tests/test_emul_racecheck.py runs the emulator tests that way)."""
     global _LIB
     if _LIB is None:
         import build_emul
-        _LIB = _native.bind(C.CDLL(build_emul.build()))
+        racecheck = os.environ.get("MGB_EMUL_BUILD", "") == "racecheck"
+        _LIB = _native.bind(C.CDLL(build_emul.build(racecheck=racecheck)))
     return _LIB
 
 
