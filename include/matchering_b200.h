@@ -206,6 +206,56 @@ int mgb_track_layout_init(const mgb_plan* plan, int64_t target_frames, int64_t r
 int mgb_match_levels(const mgb_plan* plan, const mgb_track_layout* layout, const float* d_target_lr,
                      const float* d_reference_lr, void* d_workspace, mgb_track_state* d_state, void* stream);
 
+/* ---- reference profiles: analyse a reference once, master any number of targets against it ----
+ * Everything stages 2-4 take from the reference depends on the reference and on five Config fields only
+ * (sample_rate, fft_size, max_piece_size, threshold, min_value): its peak and final_amplitude_coefficient
+ * (match_levels.py:29-44 normalize_reference), the match RMS of the normalised reference and its number of
+ * loud pieces (match_levels.py:47-71 analyze_levels), and the two average spectra of the normalised reference
+ * over its loudest pieces (match_frequencies.py:30-42,93-94 __average_fft).  A profile holds exactly those, in
+ * one device blob of mgb_reference_profile_bytes(): this header, then double spectra[2][n_lin] (mid, side:
+ * mean |rfft(frame)| / fft_size of the normalised reference over its loud pieces).  A job that takes its
+ * reference from a profile computes exactly what the job that takes the reference's samples computes: the same
+ * level statistics, c0 and FIR bit for bit, and from there on the same kernels on the same data (whose per-piece
+ * float64 atomic sums make two device runs of ONE job differ in the last bits; where the order is fixed, as in the
+ * CPU emulator, outputs and mgb_track_state are bit-identical too).  Every Config field outside the fingerprint (limiter, LOWESS,
+ * lin_log_oversampling, rms_correction_steps) may differ between the profile's Config and the job's. */
+#define MGB_REFERENCE_PROFILE_VERSION 1
+typedef struct mgb_reference_profile {
+    int32_t version;              /* MGB_REFERENCE_PROFILE_VERSION */
+    int32_t sample_rate, fft_size, n_lin;
+    double max_piece_size, threshold, min_value;    /* the Config fields the reference side depends on */
+    int64_t reference_frames, reference_piece;
+    int32_t reference_divisions, reference_loud_pieces;
+    double reference_peak;        /* max|reference|                                  */
+    double final_amplitude_coef;  /* normalize_reference's coefficient               */
+    double reference_match_rms;   /* of the NORMALISED reference                      */
+    int64_t reserved;             /* 0; the spectra follow at sizeof(mgb_reference_profile) = 96 */
+} mgb_reference_profile;
+
+/* bytes of a profile blob for this plan's fft_size (header + spectra) */
+int64_t mgb_reference_profile_bytes(const mgb_plan* plan);
+/* device scratch mgb_analyze_reference needs for a reference of `reference_frames` frames */
+int64_t mgb_reference_workspace_bytes(const mgb_plan* plan, int64_t reference_frames);
+/* One analysis pass over the reference (the pass mgb_match_levels makes over it) and its fold into a profile
+ * at d_profile (device, mgb_reference_profile_bytes).  Asynchronous on `stream`. */
+int mgb_analyze_reference(const mgb_plan* plan, const float* d_reference_lr, int64_t reference_frames, void* d_workspace,
+                          int64_t workspace_bytes, void* d_profile, void* stream);
+/* Compares a HOST copy of a profile's header with the plan: version, sample_rate, fft_size, n_lin, max_piece_size,
+ * threshold and min_value must match exactly (MGB_ERR_INVALID naming the first field that does not).  The device
+ * entry points below cannot read the device header without a synchronisation, so they trust the caller to have
+ * made this check. */
+int mgb_reference_profile_check(const mgb_plan* plan, const mgb_reference_profile* h_header);
+/* Layout of a job whose reference comes from a profile: the target's geometry as mgb_track_layout_init gives it;
+ * reference_frames, reference_piece, reference_divisions and reference_slots are 0, which marks the layout as
+ * profiled.  Its workspace has no reference regions and one region for a copy of the profile. */
+int mgb_track_layout_init_profiled(const mgb_plan* plan, int64_t target_frames, mgb_track_layout* out);
+/* Stage 1 with the reference from a profile: copies the blob into the workspace on `stream` (the caller may reuse
+ * or free d_profile once that copy has run), analyses the target, and the next stage's first kernel combines the
+ * target's statistics with the profile's.  MGB_ERR_INVALID with a paired layout, as mgb_match_levels gives with a
+ * profiled one.  Stages 2-4 take a profiled layout like a paired one. */
+int mgb_match_levels_profiled(const mgb_plan* plan, const mgb_track_layout* layout, const float* d_target_lr,
+                              const void* d_profile, void* d_workspace, mgb_track_state* d_state, void* stream);
+
 /* ---- stage 2: stages.__match_frequencies (stages.py:107-135) --------------------------------
  * FIR design for mid and side (match_frequencies.get_fir, :78-101, incl. __smooth_exponentially
  * :45-75 and dsp.smooth_lowess) and convolution of the level-matched target with both FIRs
@@ -302,6 +352,12 @@ int mgb_stages_main_host(mgb_host_io* io, const mgb_plan* plan, const mgb_track_
                          const void* h_reference, int32_t in_width, void* h_out_limited, void* h_out_no_limiter,
                          void* h_out_normalized, int32_t out_width, const mgb_host_buffers* dev,
                          mgb_track_state* h_state_out, void* stream);
+/* The same with the reference from a device profile (mgb_analyze_reference): only the target crosses the link.
+ * dev->d_reference_lr is not used and may be NULL; `layout` comes from mgb_track_layout_init_profiled. */
+int mgb_stages_main_host_profiled(mgb_host_io* io, const mgb_plan* plan, const mgb_track_layout* layout,
+                                  const void* h_target, int32_t in_width, const void* d_profile, void* h_out_limited,
+                                  void* h_out_no_limiter, void* h_out_normalized, int32_t out_width,
+                                  const mgb_host_buffers* dev, mgb_track_state* h_state_out, void* stream);
 /* limiter.limit (matchering/limiter/hyrax.py:78-99) on a host array.  *h_engaged_out = 0 means the
  * reference would return its input object untouched (hyrax.py:83-85): h_out is then NOT written. */
 int mgb_limit_host(mgb_host_io* io, const mgb_limiter_params* params, const void* h_in, int32_t in_width, void* h_out,
@@ -325,6 +381,13 @@ int mgb_pipeline_submit(mgb_pipeline* p, const float* h_target_lr, int64_t targe
 int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
                             const void* h_reference_pcm, int32_t reference_bits, int64_t reference_frames,
                             void* h_out_pcm, int32_t out_bits, int32_t* slot_out);
+/* Both with the reference from a device profile instead of reference samples: no reference bytes cross the link.
+ * d_profile must stay valid until mgb_pipeline_wait returns for the slot.  Paired and profiled submissions may be
+ * mixed in one pipeline; its slot workspace covers both. */
+int mgb_pipeline_submit_profiled(mgb_pipeline* p, const float* h_target_lr, int64_t target_frames, const void* d_profile,
+                                 float* h_out_limited, int32_t* slot_out);
+int mgb_pipeline_submit_pcm_profiled(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
+                                     const void* d_profile, void* h_out_pcm, int32_t out_bits, int32_t* slot_out);
 int mgb_pipeline_wait(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out);
 int mgb_pipeline_streams(mgb_pipeline* p, void** h2d, void** compute, void** d2h);
 int mgb_pipeline_destroy(mgb_pipeline* p);

@@ -12,6 +12,7 @@ from .results import Result, pcm16, pcm24
 from .defaults import Config, LimiterConfig
 from .loader import load
 from .checker import check
+from .profile import ReferenceProfile, analyze_reference
 
 
 def process(*args, **kwargs):

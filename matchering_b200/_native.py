@@ -119,6 +119,21 @@ class TrackLayout(C.Structure):
     ]
 
 
+MGB_REFERENCE_PROFILE_VERSION = 1
+
+
+class ReferenceProfileHeader(C.Structure):
+    """mgb_reference_profile: the header of a device profile blob; double spectra[2][n_lin] follow it."""
+    _fields_ = [
+        ("version", C.c_int32), ("sample_rate", C.c_int32), ("fft_size", C.c_int32), ("n_lin", C.c_int32),
+        ("max_piece_size", C.c_double), ("threshold", C.c_double), ("min_value", C.c_double),
+        ("reference_frames", C.c_int64), ("reference_piece", C.c_int64),
+        ("reference_divisions", C.c_int32), ("reference_loud_pieces", C.c_int32),
+        ("reference_peak", C.c_double), ("final_amplitude_coef", C.c_double), ("reference_match_rms", C.c_double),
+        ("reserved", C.c_int64),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/matchering_b200.h declares
 PROTOTYPES = {
     "mgb_version": (C.c_int, []),
@@ -134,6 +149,21 @@ PROTOTYPES = {
     "mgb_track_layout_init": (C.c_int, [C.POINTER(Plan), C.c_int64, C.c_int64, C.POINTER(TrackLayout)]),
     "mgb_match_levels": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p]),
+    "mgb_reference_profile_bytes": (C.c_int64, [C.POINTER(Plan)]),
+    "mgb_reference_workspace_bytes": (C.c_int64, [C.POINTER(Plan), C.c_int64]),
+    "mgb_analyze_reference": (C.c_int, [C.POINTER(Plan), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_void_p]),
+    "mgb_reference_profile_check": (C.c_int, [C.POINTER(Plan), C.POINTER(ReferenceProfileHeader)]),
+    "mgb_track_layout_init_profiled": (C.c_int, [C.POINTER(Plan), C.c_int64, C.POINTER(TrackLayout)]),
+    "mgb_match_levels_profiled": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p]),
+    "mgb_stages_main_host_profiled": (C.c_int, [C.c_void_p, C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_int32,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                                C.POINTER(HostBuffers), C.POINTER(TrackState), C.c_void_p]),
+    "mgb_pipeline_submit_profiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                               C.POINTER(C.c_int32)]),
+    "mgb_pipeline_submit_pcm_profiled": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                                   C.c_int32, C.POINTER(C.c_int32)]),
     "mgb_match_frequencies": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_correct_levels": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p]),

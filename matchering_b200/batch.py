@@ -15,10 +15,14 @@ import torch
 
 from . import _native
 from .engine import get_plan
+from .profile import ReferenceProfile
 
 
 class MasteringPipeline:
     def __init__(self, config, max_target_frames: int, max_reference_frames: int, depth: int = 3, device=None):
+        """max_reference_frames bounds the references submitted as samples; profiles have no such bound
+        (a pipeline that only takes profiles may pass smallest_reference_frames(config))."""
+        self.config = config
         self.plan = get_plan(config, device)
         self.lib = self.plan.lib
         self.device = self.plan.device
@@ -37,14 +41,26 @@ class MasteringPipeline:
         assert a.dtype == np.float32 and a.flags["C_CONTIGUOUS"]
         return a.ctypes.data, a.shape[0]
 
+    def _profile_blob(self, profile: ReferenceProfile):
+        profile.check_config(self.config)
+        return profile.checked_blob(self.plan)
+
     def submit(self, target, reference, out) -> int:
         """target, reference, out: (frames, 2) float32 host arrays (numpy or torch, ideally pinned).
+        `reference` may be a ReferenceProfile: then no reference bytes are copied.
         Returns the slot to `wait` on; `out` is valid once that wait returns."""
         tp, tn = self._ptr(target)
-        rp, rn = self._ptr(reference)
         op, on = self._ptr(out)
         assert on == tn
         slot = C.c_int32()
+        if isinstance(reference, ReferenceProfile):
+            blob = self._profile_blob(reference)
+            with torch.cuda.device(self.device):
+                _native.check(self.lib, self.lib.mgb_pipeline_submit_profiled(self._handle, tp, tn, blob.data_ptr(), op,
+                                                                              C.byref(slot)))
+            self._pending[slot.value] = (target, blob, out)
+            return slot.value
+        rp, rn = self._ptr(reference)
         with torch.cuda.device(self.device):
             _native.check(self.lib, self.lib.mgb_pipeline_submit(self._handle, tp, tn, rp, rn, op, C.byref(slot)))
         self._pending[slot.value] = (target, reference, out)
@@ -65,10 +81,17 @@ class MasteringPipeline:
             assert a_np.flags["C_CONTIGUOUS"]
             return a_np.ctypes.data, bits, a_np.shape[0]
         tp, tb, tn = describe(target)
-        rp, rb, rn = describe(reference)
         op, ob, on = describe(out)
         assert on == tn
         slot = C.c_int32()
+        if isinstance(reference, ReferenceProfile):
+            blob = self._profile_blob(reference)
+            with torch.cuda.device(self.device):
+                _native.check(self.lib, self.lib.mgb_pipeline_submit_pcm_profiled(self._handle, tp, tb, tn, blob.data_ptr(),
+                                                                                  op, ob, C.byref(slot)))
+            self._pending[slot.value] = (target, blob, out)
+            return slot.value
+        rp, rb, rn = describe(reference)
         with torch.cuda.device(self.device):
             _native.check(self.lib, self.lib.mgb_pipeline_submit_pcm(self._handle, tp, tb, tn, rp, rb, rn, op, ob,
                                                                      C.byref(slot)))
@@ -103,16 +126,27 @@ class MasteringPipeline:
         self.close()
 
 
+def smallest_reference_frames(config) -> int:
+    """The shortest reference a pipeline can be created for: one piece just longer than fft_size."""
+    return int(config.fft_size) + 1
+
+
 def master_many(pairs, config, depth: int = 3):
-    """[(target, reference), ...] float32 host arrays -> list of limited results (numpy float32)."""
+    """[(target, reference), ...] float32 host arrays -> list of limited results (numpy float32).  A reference
+    may be a ReferenceProfile (an album against one reference: analysed once, never copied again)."""
     pairs = list(pairs)
     if not pairs:
         return []
+    for _, r in pairs:  # a Config the profile was not made for fails before any device work
+        if isinstance(r, ReferenceProfile):
+            r.check_config(config)
     max_t = max(len(t) for t, _ in pairs)
-    max_r = max(len(r) for _, r in pairs)
+    max_r = max((len(r) for _, r in pairs if not isinstance(r, ReferenceProfile)), default=smallest_reference_frames(config))
     outs = [np.empty((len(t), 2), dtype=np.float32) for t, _ in pairs]
     with MasteringPipeline(config, max_t, max_r, depth) as pipe:
         for (t, r), o in zip(pairs, outs):
-            pipe.submit(np.ascontiguousarray(t, dtype=np.float32), np.ascontiguousarray(r, dtype=np.float32), o)
+            if not isinstance(r, ReferenceProfile):
+                r = np.ascontiguousarray(r, dtype=np.float32)
+            pipe.submit(np.ascontiguousarray(t, dtype=np.float32), r, o)
         pipe.wait_all()
     return outs

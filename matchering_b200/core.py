@@ -4,6 +4,7 @@ from .checker import check, check_equality
 from .defaults import Config
 from .loader import load
 from .log import Code, ModuleError, debug, debug_line, info
+from .profile import ReferenceProfile
 from .results import Result
 from .saver import save
 from .stages import main_device
@@ -12,8 +13,11 @@ from .utils import get_temp_folder
 _DEFAULT_CONFIG = None
 
 
-def process(target: str, reference: str, results: list, config: Config = None,
+def process(target: str, reference, results: list, config: Config = None,
             preview_target: Result = None, preview_result: Result = None):
+    """`reference` is a file path or a ReferenceProfile (mg.analyze_reference): mastering many targets against
+    one reference analyses it once.  With a profile the allow_equality check has no reference samples to
+    compare with and is skipped."""
     global _DEFAULT_CONFIG
     if config is None:
         if _DEFAULT_CONFIG is None:
@@ -25,14 +29,26 @@ def process(target: str, reference: str, results: list, config: Config = None,
         raise RuntimeError("The result list is empty")
     temp_folder = config.temp_folder if config.temp_folder else get_temp_folder(results)
 
-    target_audio, target_rate = _load_and_check(target, "target", temp_folder, config)
-    reference_audio, reference_rate = _load_and_check(reference, "reference", temp_folder, config)
-    if not config.allow_equality:
-        _check_equality_any(target_audio, reference_audio)
-    if (not (target_rate == reference_rate == config.internal_sample_rate)
-            or not (target_audio.shape[1] == reference_audio.shape[1] == 2)
-            or not (target_audio.shape[0] > config.fft_size and reference_audio.shape[0] > config.fft_size)):
-        raise ModuleError(Code.ERROR_VALIDATION)
+    if isinstance(reference, ReferenceProfile):
+        # the reference was loaded, checked and analysed when the profile was made; only its fingerprint is
+        # compared with this Config here.  There are no reference samples to compare the target with.
+        reference.check_config(config)
+        target_audio, target_rate = _load_and_check(target, "target", temp_folder, config)
+        if not config.allow_equality:
+            debug("The REFERENCE is a profile: the check that the TARGET differs from it is skipped")
+        if (target_rate != config.internal_sample_rate or target_audio.shape[1] != 2
+                or not target_audio.shape[0] > config.fft_size):
+            raise ModuleError(Code.ERROR_VALIDATION)
+        reference_audio = reference
+    else:
+        target_audio, target_rate = _load_and_check(target, "target", temp_folder, config)
+        reference_audio, reference_rate = _load_and_check(reference, "reference", temp_folder, config)
+        if not config.allow_equality:
+            _check_equality_any(target_audio, reference_audio)
+        if (not (target_rate == reference_rate == config.internal_sample_rate)
+                or not (target_audio.shape[1] == reference_audio.shape[1] == 2)
+                or not (target_audio.shape[0] > config.fft_size and reference_audio.shape[0] > config.fft_size)):
+            raise ModuleError(Code.ERROR_VALIDATION)
 
     limited, plain, normalized = main_device(
         target_audio, reference_audio, config,

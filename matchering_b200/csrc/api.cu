@@ -121,8 +121,33 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     w.lookback = take(limiter_lookback_bytes(plan.limiter, L.target_frames));
     w.limiter_zero_bytes = off - limiter_zero_from;
     w.limiter_planes = take(limiter_plane_bytes(plan.limiter, L.target_frames));  // (empty unless the wide-window path runs)
+    // a profiled layout (no reference pieces): the copy of the profile, behind everything a paired layout has
+    w.profile = L.reference_divisions == 0 ? (const mgb_reference_profile*)take(reference_profile_bytes(plan)) : nullptr;
     w.total_bytes = off;
     return w;
+}
+
+static bool layout_profiled(const mgb_track_layout& L) {
+    return L.reference_divisions == 0 && L.reference_slots == 0 && L.reference_piece == 0;
+}
+
+// mgb_analyze_reference's scratch; with base_ptr == nullptr the pointers hold byte offsets
+static ReferenceRegions carve_reference(const mgb_plan& plan, const ReferenceGeometry& g, void* base_ptr) {
+    ReferenceRegions r;
+    const uintptr_t base = reinterpret_cast<uintptr_t>(base_ptr);
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) {
+        unsigned char* p = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
+        off += align256(bytes);
+        return p;
+    };
+    const int64_t items = (int64_t)g.divisions * g.slots;
+    r.spec_part = (float*)take(items * 2 * plan.n_lin * 4);
+    r.sumsq_part = (double*)take(items * 8);
+    r.absmax_part = (float*)take((items + 1) * 4);
+    r.mask = take(g.divisions);
+    r.total_bytes = off;
+    return r;
 }
 
 static int check_plan(const mgb_plan* plan) {
@@ -437,6 +462,30 @@ int mgb_plan_build_operator(const mgb_plan* plan, double* d_operator_out, void* 
     return build_operator(*plan, d_operator_out, d_workspace, (cudaStream_t)stream);
 }
 
+// match_levels.py:47-59 piece geometry of one signal of n frames (n > fft_size and max_piece_size > 0 checked by the
+// caller), and its analysis work items
+static int signal_geometry(const mgb_plan* plan, int64_t n, ReferenceGeometry* g) {
+    // match_levels.py:47-59: float division, then int() truncation
+    const double q = (double)n / plan->max_piece_size;
+    MGB_REQUIRE(q < 8000.0, MGB_ERR_UNSUPPORTED, "more than 8000 pieces (their statistics live in one CTA's shared memory)");
+    const int32_t divisions = (int32_t)q + 1;
+    const int64_t piece = (int64_t)((double)n / (double)divisions);
+    MGB_REQUIRE(piece >= plan->fft_size, MGB_ERR_UNSUPPORTED,
+                "piece of %lld samples is shorter than fft_size %d (the reference's STFT degenerates there)",
+                (long long)piece, plan->fft_size);
+    const int64_t frames_per_piece = piece / plan->fft_size;
+    // analysis work items: one wave of three resident CTAs per SM (register/shared-memory limit of
+    // analyze_kernel), never more items than that so that no tail wave forms
+    int64_t slots = (3LL * num_sms()) / divisions;
+    if (slots > frames_per_piece) slots = frames_per_piece;
+    if (slots < 1) slots = 1;
+    g->frames = n;
+    g->piece = piece;
+    g->divisions = divisions;
+    g->slots = (int32_t)slots;
+    return MGB_OK;
+}
+
 int mgb_track_layout_init(const mgb_plan* plan, int64_t target_frames, int64_t reference_frames,
                           mgb_track_layout* out) {
     MGB_TRY(check_plan(plan));
@@ -447,43 +496,122 @@ int mgb_track_layout_init(const mgb_plan* plan, int64_t target_frames, int64_t r
                 (long long)reference_frames, plan->fft_size);
     MGB_REQUIRE(plan->max_piece_size > 0, MGB_ERR_INVALID, "max_piece_size must be positive");
     memset(out, 0, sizeof(*out));
+    ReferenceGeometry t, r;
+    MGB_TRY(signal_geometry(plan, target_frames, &t));
+    MGB_TRY(signal_geometry(plan, reference_frames, &r));
     out->target_frames = target_frames;
     out->reference_frames = reference_frames;
-    const int sms = num_sms();
-    for (int sig = 0; sig < 2; ++sig) {
-        const int64_t n = sig == 0 ? target_frames : reference_frames;
-        // match_levels.py:47-59: float division, then int() truncation
-        const double q = (double)n / plan->max_piece_size;
-        MGB_REQUIRE(q < 8000.0, MGB_ERR_UNSUPPORTED, "more than 8000 pieces (their statistics live in one CTA's shared memory)");
-        const int32_t divisions = (int32_t)q + 1;
-        const int64_t piece = (int64_t)((double)n / (double)divisions);
-        MGB_REQUIRE(piece >= plan->fft_size, MGB_ERR_UNSUPPORTED,
-                    "piece of %lld samples is shorter than fft_size %d (the reference's STFT degenerates there)",
-                    (long long)piece, plan->fft_size);
-        const int64_t frames_per_piece = piece / plan->fft_size;
-        // analysis work items: one wave of three resident CTAs per SM (register/shared-memory limit of
-        // analyze_kernel), never more items than that so that no tail wave forms
-        int64_t slots = (3LL * sms) / divisions;
-        if (slots > frames_per_piece) slots = frames_per_piece;
-        if (slots < 1) slots = 1;
-        if (sig == 0) {
-            out->target_divisions = divisions;
-            out->target_piece = piece;
-            out->target_slots = (int32_t)slots;
-        } else {
-            out->reference_divisions = divisions;
-            out->reference_piece = piece;
-            out->reference_slots = (int32_t)slots;
-        }
-    }
+    out->target_divisions = t.divisions;
+    out->target_piece = t.piece;
+    out->target_slots = t.slots;
+    out->reference_divisions = r.divisions;
+    out->reference_piece = r.piece;
+    out->reference_slots = r.slots;
     out->workspace_bytes = carve_workspace(*plan, *out, nullptr).total_bytes;
     return MGB_OK;
+}
+
+int mgb_track_layout_init_profiled(const mgb_plan* plan, int64_t target_frames, mgb_track_layout* out) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(out != nullptr, MGB_ERR_INVALID, "layout is NULL");
+    MGB_REQUIRE(target_frames > plan->fft_size, MGB_ERR_INVALID, "target (%lld) must be longer than fft_size (%d)",
+                (long long)target_frames, plan->fft_size);
+    MGB_REQUIRE(plan->max_piece_size > 0, MGB_ERR_INVALID, "max_piece_size must be positive");
+    memset(out, 0, sizeof(*out));
+    ReferenceGeometry t;
+    MGB_TRY(signal_geometry(plan, target_frames, &t));
+    out->target_frames = target_frames;
+    out->target_divisions = t.divisions;
+    out->target_piece = t.piece;
+    out->target_slots = t.slots;
+    out->workspace_bytes = carve_workspace(*plan, *out, nullptr).total_bytes;
+    return MGB_OK;
+}
+
+int64_t mgb_reference_profile_bytes(const mgb_plan* plan) {
+    if (check_plan(plan) != MGB_OK) return -1;
+    return reference_profile_bytes(*plan);
+}
+
+static int reference_geometry(const mgb_plan* plan, int64_t reference_frames, ReferenceGeometry* g) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(reference_frames > plan->fft_size, MGB_ERR_INVALID, "reference (%lld) must be longer than fft_size (%d)",
+                (long long)reference_frames, plan->fft_size);
+    MGB_REQUIRE(plan->max_piece_size > 0, MGB_ERR_INVALID, "max_piece_size must be positive");
+    return signal_geometry(plan, reference_frames, g);
+}
+
+int64_t mgb_reference_workspace_bytes(const mgb_plan* plan, int64_t reference_frames) {
+    ReferenceGeometry g;
+    if (reference_geometry(plan, reference_frames, &g) != MGB_OK) return -1;
+    return carve_reference(*plan, g, nullptr).total_bytes;
+}
+
+int mgb_analyze_reference(const mgb_plan* plan, const float* d_reference_lr, int64_t reference_frames, void* d_workspace,
+                          int64_t workspace_bytes, void* d_profile, void* stream) {
+    ReferenceGeometry g;
+    MGB_TRY(reference_geometry(plan, reference_frames, &g));
+    MGB_TRY(check_aligned(d_reference_lr, "d_reference_lr"));
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_profile, "d_profile"));
+    const ReferenceRegions need = carve_reference(*plan, g, nullptr);
+    MGB_REQUIRE(workspace_bytes >= need.total_bytes, MGB_ERR_WORKSPACE, "analyze_reference: workspace of %lld bytes, need %lld",
+                (long long)workspace_bytes, (long long)need.total_bytes);
+    cudaStream_t st = (cudaStream_t)stream;
+    const ReferenceRegions r = carve_reference(*plan, g, d_workspace);
+    MGB_TRY(launch_analyze(*plan, (const float2*)d_reference_lr, g.frames, g.piece, g.divisions, g.slots, r.spec_part,
+                           r.sumsq_part, r.absmax_part, st));
+    return launch_reference_profile(*plan, g, r, (mgb_reference_profile*)d_profile, st);
+}
+
+int mgb_reference_profile_check(const mgb_plan* plan, const mgb_reference_profile* h) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(h != nullptr, MGB_ERR_INVALID, "profile header is NULL");
+    MGB_REQUIRE(h->version == MGB_REFERENCE_PROFILE_VERSION, MGB_ERR_INVALID, "reference profile: version %d, this library reads %d",
+                h->version, MGB_REFERENCE_PROFILE_VERSION);
+#define MGB_PROFILE_FIELD(field, fmt, cast)                                                                             \
+    MGB_REQUIRE(h->field == plan->field, MGB_ERR_INVALID, "reference profile: " #field " " fmt " differs from the Config's " fmt, \
+                (cast)h->field, (cast)plan->field)
+    MGB_PROFILE_FIELD(sample_rate, "%d", int);
+    MGB_PROFILE_FIELD(fft_size, "%d", int);
+    MGB_PROFILE_FIELD(n_lin, "%d", int);
+    MGB_PROFILE_FIELD(max_piece_size, "%.17g", double);
+    MGB_PROFILE_FIELD(threshold, "%.17g", double);
+    MGB_PROFILE_FIELD(min_value, "%.17g", double);
+#undef MGB_PROFILE_FIELD
+    return MGB_OK;
+}
+
+int mgb_match_levels_profiled(const mgb_plan* plan, const mgb_track_layout* L, const float* d_target_lr, const void* d_profile,
+                              void* d_workspace, mgb_track_state* d_state, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_REQUIRE(layout_profiled(*L), MGB_ERR_INVALID,
+                "match_levels_profiled: the layout has reference pieces (use mgb_track_layout_init_profiled)");
+    MGB_TRY(check_aligned(d_target_lr, "d_target_lr"));
+    MGB_TRY(check_aligned(d_profile, "d_profile"));
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    cudaStream_t st = (cudaStream_t)stream;
+    Workspace ws = carve_workspace(*plan, *L, d_workspace);
+    const size_t pbytes = (size_t)reference_profile_bytes(*plan);
+#ifdef MGB_EMULATE
+    memset(ws.zero_begin, 0, ws.zero_end - ws.zero_begin);
+    memcpy((void*)ws.profile, d_profile, pbytes);
+#else
+    if (cudaMemsetAsync(ws.zero_begin, 0, ws.zero_end - ws.zero_begin, st) != cudaSuccess) return cuda_status("memset");
+    if (cudaMemcpyAsync((void*)ws.profile, d_profile, pbytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+        return cuda_status("profile copy");
+#endif
+    return launch_analyze(*plan, (const float2*)d_target_lr, L->target_frames, L->target_piece, L->target_divisions,
+                          L->target_slots, ws.spec_part_t, ws.sumsq_part_t, ws.absmax_part_t, st);
 }
 
 int mgb_match_levels(const mgb_plan* plan, const mgb_track_layout* L, const float* d_target_lr,
                      const float* d_reference_lr, void* d_workspace, mgb_track_state* d_state, void* stream) {
     MGB_TRY(check_plan(plan));
     MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_REQUIRE(!layout_profiled(*L), MGB_ERR_INVALID,
+                "match_levels: the layout is profiled (its reference comes from mgb_match_levels_profiled)");
     MGB_TRY(check_aligned(d_target_lr, "d_target_lr"));
     MGB_TRY(check_aligned(d_reference_lr, "d_reference_lr"));
     MGB_TRY(check_aligned(d_workspace, "d_workspace"));

@@ -352,9 +352,23 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 
 constexpr int kMeanBins = 32, kMeanSlices = 32;
 
+// What one spectrum-mean launch folds.  kPaired: target and reference partials into the matching curve.
+// kProfiled: the target's partials, the reference half from a profile (mgb_match_levels_profiled).  kProfile: the
+// reference's partials alone into a profile (mgb_analyze_reference; div_t = 0).  The halves that exist run the
+// same code in every mode, so a profile holds exactly the reference terms a paired job computes, bit for bit.
+enum class MeanMode { kPaired, kProfiled, kProfile };
+
+struct ProfileIO {
+    const mgb_reference_profile* in;  // kProfiled: the profile (header, then spectra [2][n_lin])
+    mgb_reference_profile* out;       // kProfile: where the profile goes
+    mgb_reference_profile header;     // kProfile: its fingerprint and geometry, filled by the host
+};
+
+template <MeanMode MODE>
 __global__ void __launch_bounds__(kMeanBins * kMeanSlices)
-spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, PrefetchList pf) {
+spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, PrefetchList pf, ProfileIO io) {
     constexpr int BINS = kMeanBins, SLICES = kMeanSlices;
+    constexpr bool kHasT = MODE != MeanMode::kProfile, kHasR = MODE != MeanMode::kProfiled;
     __shared__ double part_t[SLICES][BINS + 1], part_r[SLICES][BINS + 1];
     MGB_DYN_SMEM(smem);  // loudest-piece masks: [div_t] then [div_r] bytes
     unsigned char* mask_t = smem;
@@ -380,11 +394,13 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
         if (threadIdx.x == 0) peak_bits_s = target_peak_bits_s = 0u;
         __syncthreads();
-        float pk = 0.0f;
-        for (int i = threadIdx.x; i < a.div_r * a.slots_r + 1; i += blockDim.x) pk = fmaxf(pk, a.levels.absmax_r[i]);
-        pk = warp_max_f(pk);
-        if (lane == 0 && pk > 0.0f) atomicMax(&peak_bits_s, __float_as_uint(pk));  // non-negative floats order like their bits
-        if (blockIdx.x == 0 && blockIdx.y == 0) {  // the target's peak: the convolution's choice of precision needs it
+        if constexpr (kHasR) {
+            float pk = 0.0f;
+            for (int i = threadIdx.x; i < a.div_r * a.slots_r + 1; i += blockDim.x) pk = fmaxf(pk, a.levels.absmax_r[i]);
+            pk = warp_max_f(pk);
+            if (lane == 0 && pk > 0.0f) atomicMax(&peak_bits_s, __float_as_uint(pk));  // non-negative floats order like their bits
+        }
+        if (kHasT && blockIdx.x == 0 && blockIdx.y == 0) {  // the target's peak: the convolution's choice of precision needs it
             float tpk = 0.0f;
             for (int i = threadIdx.x; i < a.div_t * a.slots_t + 1; i += blockDim.x) tpk = fmaxf(tpk, a.absmax_t[i]);
             tpk = warp_max_f(tpk);
@@ -402,14 +418,36 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
         }
         __syncthreads();
         if (threadIdx.x < 32) {
-            LevelsArgs folded = a.levels;
-            folded.sumsq_t = piece_sum;
-            folded.sumsq_r = piece_sum + a.div_t;
-            folded.slots_t = folded.slots_r = 1;
-            const float peak = __uint_as_float(peak_bits_s);
-            folded.absmax_r = &peak;
-            folded.div_r_items_override = 1;
-            const LevelsResult mine = levels_compute_warp(folded, mask_t, mask_r);
+            LevelsResult mine;
+            if constexpr (MODE == MeanMode::kPaired) {
+                LevelsArgs folded = a.levels;
+                folded.sumsq_t = piece_sum;
+                folded.sumsq_r = piece_sum + a.div_t;
+                folded.slots_t = folded.slots_r = 1;
+                const float peak = __uint_as_float(peak_bits_s);
+                folded.absmax_r = &peak;
+                folded.div_r_items_override = 1;
+                mine = levels_compute_warp(folded, mask_t, mask_r);
+            } else if constexpr (MODE == MeanMode::kProfiled) {  // levels_compute_warp's target half, the rest recorded
+                const SignalLevels t = signal_levels_warp(piece_sum, a.div_t, 1, (double)a.levels.piece_t, mask_t);
+                mine.peak = io.in->reference_peak;
+                mine.coef = io.in->final_amplitude_coef;
+                mine.match_t = t.match;
+                mine.match_r = io.in->reference_match_rms;
+                mine.c0 = mine.match_r / fmax(a.levels.eps, mine.match_t);
+                mine.loud_t = t.loud;
+                mine.loud_r = io.in->reference_loud_pieces;
+            } else {  // levels_compute_warp's reference half
+                const float peak = __uint_as_float(peak_bits_s);
+                mine.peak = (double)warp_max_f(lane == 0 ? fmaxf(0.0f, peak) : 0.0f);
+                mine.coef = reference_coef(mine.peak, a.levels.threshold, a.levels.eps);
+                const SignalLevels r = signal_levels_warp(piece_sum, a.div_r, 1, (double)a.levels.piece_r, mask_r);
+                mine.match_t = 0.0;
+                mine.match_r = r.match / mine.coef;
+                mine.c0 = 0.0;
+                mine.loud_t = 0;
+                mine.loud_r = r.loud;
+            }
             if (threadIdx.x == 0) lv_s = mine;
         }
     }
@@ -417,12 +455,21 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
     const LevelsResult lv = lv_s;
     if (blockIdx.x == 0 && blockIdx.y == 0) {
         if (threadIdx.x == 0) {
-            levels_store(lv, a.state);
-            a.state->conv_peak_bits = 0.0f;
-            a.state->fir_peak_mid_bits = 0.0f;
-            a.state->fir_peak_side_bits = 0.0f;
-            a.state->conv_precise = 0;
-            *a.target_peak = __uint_as_float(target_peak_bits_s);
+            if constexpr (kHasT) {
+                levels_store(lv, a.state);
+                a.state->conv_peak_bits = 0.0f;
+                a.state->fir_peak_mid_bits = 0.0f;
+                a.state->fir_peak_side_bits = 0.0f;
+                a.state->conv_precise = 0;
+                *a.target_peak = __uint_as_float(target_peak_bits_s);
+            } else {
+                mgb_reference_profile h = io.header;
+                h.reference_loud_pieces = lv.loud_r;
+                h.reference_peak = lv.peak;
+                h.final_amplitude_coef = lv.coef;
+                h.reference_match_rms = lv.match_r;
+                *io.out = h;
+            }
         }
         for (int p = threadIdx.x; p < a.div_t; p += blockDim.x) a.mask_t[p] = mask_t[p];
         for (int p = threadIdx.x; p < a.div_r; p += blockDim.x) a.mask_r[p] = mask_r[p];
@@ -483,8 +530,8 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
             }
             return total;
         };
-        st = selected_sum(a.spec_part_t, sel, n_sel_s[0]);
-        sr = selected_sum(a.spec_part_r, sel + a.div_t * a.slots_t, n_sel_s[1]);
+        if constexpr (kHasT) st = selected_sum(a.spec_part_t, sel, n_sel_s[0]);
+        if constexpr (kHasR) sr = selected_sum(a.spec_part_r, sel + a.div_t * a.slots_t, n_sel_s[1]);
     }
     part_t[sy][bx] = st;
     part_r[sy][bx] = sr;
@@ -498,7 +545,14 @@ spectrum_mean_kernel(DesignArgs a, int n_lin, int fft_size, double eps, Prefetch
         // normalisation 1/coef are applied to the means instead of to the samples
         const double norm_t = lv.c0 / ((double)lv.loud_t * (double)a.frames_per_piece_t * (double)fft_size);
         const double norm_r = 1.0 / (lv.coef * (double)lv.loud_r * (double)a.frames_per_piece_r * (double)fft_size);
-        a.scratch[(long long)(kDesignBlocks * ch) * a.stride + k] = (sr * norm_r) / fmax(eps, st * norm_t);
+        if constexpr (MODE == MeanMode::kPaired) {
+            a.scratch[(long long)(kDesignBlocks * ch) * a.stride + k] = (sr * norm_r) / fmax(eps, st * norm_t);
+        } else if constexpr (MODE == MeanMode::kProfiled) {
+            const double* spectra = reinterpret_cast<const double*>(io.in + 1);
+            a.scratch[(long long)(kDesignBlocks * ch) * a.stride + k] = spectra[(long long)ch * n_lin + k] / fmax(eps, st * norm_t);
+        } else {
+            reinterpret_cast<double*>(io.out + 1)[(long long)ch * n_lin + k] = sr * norm_r;
+        }
     }
 }
 
@@ -708,6 +762,11 @@ smooth_operator_kernel(const double* __restrict__ S, const int4* __restrict__ ro
     }
 }
 
+// dynamic shared memory of spectrum_mean_kernel: both masks, the per-piece sums and the two item lists
+size_t spectrum_mean_smem(int div_t, int64_t items_t, int div_r, int64_t items_r) {
+    return (size_t)((div_t + div_r + 15) / 16 * 16 + (int64_t)(div_t + div_r) * 8 + (items_t + items_r) * 2 + 16);
+}
+
 template <int F>
 int launch_design_t(const mgb_plan& plan, const DesignArgs& a, cudaStream_t stream) {
     return launch("design_kernel", design_kernel<F>, dim3(2 * a.ovs), dim3(kDesignThreads), DesignSmem<F>::kBytes, stream, plan, a);
@@ -803,14 +862,20 @@ int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Wo
         add(plan.d_lw_alpha, ng * 8);
         add(plan.d_lw_rows, (long long)plan.lowess_nrows * plan.lowess_k * 8);
         add(plan.d_hann, F * 8);
-        MGB_TRY(launch("spectrum_mean_kernel", spectrum_mean_kernel, dim3((plan.n_lin + kMeanBins - 1) / kMeanBins, 2),
-                       dim3(kMeanBins * kMeanSlices),
-                       (size_t)((layout.target_divisions + layout.reference_divisions + 15) / 16 * 16 +
-                                (layout.target_divisions + layout.reference_divisions) * 8 +
-                                ((int64_t)layout.target_divisions * layout.target_slots +
-                                 (int64_t)layout.reference_divisions * layout.reference_slots) * 2 + 16),
-                       stream, a, plan.n_lin,
-                       plan.fft_size, plan.min_value, pf));
+        const dim3 grid((plan.n_lin + kMeanBins - 1) / kMeanBins, 2);
+        const size_t smem = spectrum_mean_smem(layout.target_divisions, (int64_t)layout.target_divisions * layout.target_slots,
+                                               layout.reference_divisions,
+                                               (int64_t)layout.reference_divisions * layout.reference_slots);
+        ProfileIO io;
+        memset(&io, 0, sizeof(io));
+        if (ws.profile) {  // a profiled layout: the reference half comes from the workspace's copy of the profile
+            io.in = ws.profile;
+            MGB_TRY(launch("spectrum_mean_profiled_kernel", spectrum_mean_kernel<MeanMode::kProfiled>, grid,
+                           dim3(kMeanBins * kMeanSlices), smem, stream, a, plan.n_lin, plan.fft_size, plan.min_value, pf, io));
+        } else {
+            MGB_TRY(launch("spectrum_mean_kernel", spectrum_mean_kernel<MeanMode::kPaired>, grid, dim3(kMeanBins * kMeanSlices),
+                           smem, stream, a, plan.n_lin, plan.fft_size, plan.min_value, pf, io));
+        }
     }
     if (plan.d_smooth_op && plan.d_smooth_op_rows && !(avg_override && g_design_direct)) {
         if (avg_override) {
@@ -834,6 +899,44 @@ int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Wo
     }
     set_error("design: fft_size %d has no kernel", plan.fft_size);
     return MGB_ERR_UNSUPPORTED;
+}
+
+int launch_reference_profile(const mgb_plan& plan, const ReferenceGeometry& g, const ReferenceRegions& r,
+                             mgb_reference_profile* out, cudaStream_t stream) {
+    DesignArgs a;
+    memset(&a, 0, sizeof(a));
+    a.spec_part_r = r.spec_part;
+    a.mask_r = r.mask;
+    a.levels.sumsq_r = r.sumsq_part;
+    a.levels.absmax_r = r.absmax_part;
+    a.levels.piece_r = g.piece;
+    a.levels.div_r = g.divisions;
+    a.levels.slots_r = g.slots;
+    a.levels.threshold = plan.threshold;
+    a.levels.eps = plan.min_value;
+    a.div_r = g.divisions;
+    a.slots_r = g.slots;
+    a.frames_per_piece_r = g.piece / plan.fft_size;
+    PrefetchList pf;
+    memset(&pf, 0, sizeof(pf));
+    ProfileIO io;
+    memset(&io, 0, sizeof(io));
+    io.out = out;
+    mgb_reference_profile& h = io.header;
+    h.version = MGB_REFERENCE_PROFILE_VERSION;
+    h.sample_rate = plan.sample_rate;
+    h.fft_size = plan.fft_size;
+    h.n_lin = plan.n_lin;
+    h.max_piece_size = plan.max_piece_size;
+    h.threshold = plan.threshold;
+    h.min_value = plan.min_value;
+    h.reference_frames = g.frames;
+    h.reference_piece = g.piece;
+    h.reference_divisions = g.divisions;
+    return launch("reference_profile_kernel", spectrum_mean_kernel<MeanMode::kProfile>,
+                  dim3((plan.n_lin + kMeanBins - 1) / kMeanBins, 2), dim3(kMeanBins * kMeanSlices),
+                  spectrum_mean_smem(0, 0, g.divisions, (int64_t)g.divisions * g.slots), stream, a, plan.n_lin, plan.fft_size,
+                  plan.min_value, pf, io);
 }
 
 }  // namespace mgb

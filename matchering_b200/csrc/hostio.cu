@@ -627,6 +627,10 @@ int mgb_host_download(mgb_host_io* io, const float* d_src, void* h_dst, int32_t 
     return download(io, d_src, h_dst, dst_width, samples, d_wide, (cudaStream_t)stream);
 }
 
+static int stages_after_levels(mgb_host_io* io, const mgb_plan* plan, const mgb_track_layout* L, void* h_out_limited,
+                               void* h_out_no_limiter, void* h_out_normalized, int32_t out_width, const mgb_host_buffers* dev,
+                               mgb_track_state* h_state_out, cudaStream_t st);
+
 int mgb_stages_main_host(mgb_host_io* io, const mgb_plan* plan, const mgb_track_layout* L, const void* h_target,
                          const void* h_reference, int32_t in_width, void* h_out_limited, void* h_out_no_limiter,
                          void* h_out_normalized, int32_t out_width, const mgb_host_buffers* dev,
@@ -639,6 +643,29 @@ int mgb_stages_main_host(mgb_host_io* io, const mgb_plan* plan, const mgb_track_
     const UploadPiece both[2] = {{h_target, dev->d_target_lr, L->target_frames * 2}, {h_reference, dev->d_reference_lr, L->reference_frames * 2}};
     MGB_TRY(upload(io, both, 2, in_width, st));
     MGB_TRY(mgb_match_levels(plan, L, dev->d_target_lr, dev->d_reference_lr, dev->d_workspace, dev->d_state, stream));
+    return stages_after_levels(io, plan, L, h_out_limited, h_out_no_limiter, h_out_normalized, out_width, dev, h_state_out, st);
+}
+
+int mgb_stages_main_host_profiled(mgb_host_io* io, const mgb_plan* plan, const mgb_track_layout* L, const void* h_target,
+                                  int32_t in_width, const void* d_profile, void* h_out_limited, void* h_out_no_limiter,
+                                  void* h_out_normalized, int32_t out_width, const mgb_host_buffers* dev,
+                                  mgb_track_state* h_state_out, void* stream) {
+    MGB_REQUIRE(io && plan && L && h_target && d_profile && dev, MGB_ERR_INVALID, "stages_main_host_profiled: NULL argument");
+    MGB_REQUIRE(h_out_limited || h_out_no_limiter || h_out_normalized, MGB_ERR_INVALID, "no output requested");
+    MGB_REQUIRE(dev->d_target_lr && dev->d_result_lr && dev->d_out_lr && dev->d_workspace && dev->d_state, MGB_ERR_INVALID,
+                "stages_main_host_profiled: device staging buffer missing");
+    cudaStream_t st = (cudaStream_t)stream;
+    const UploadPiece target{h_target, dev->d_target_lr, L->target_frames * 2};
+    MGB_TRY(upload(io, &target, 1, in_width, st));
+    MGB_TRY(mgb_match_levels_profiled(plan, L, dev->d_target_lr, d_profile, dev->d_workspace, dev->d_state, stream));
+    return stages_after_levels(io, plan, L, h_out_limited, h_out_no_limiter, h_out_normalized, out_width, dev, h_state_out, st);
+}
+
+// stages 2-4 and the downloads of mgb_stages_main_host(_profiled), once stage 1 is on the stream
+static int stages_after_levels(mgb_host_io* io, const mgb_plan* plan, const mgb_track_layout* L, void* h_out_limited,
+                               void* h_out_no_limiter, void* h_out_normalized, int32_t out_width, const mgb_host_buffers* dev,
+                               mgb_track_state* h_state_out, cudaStream_t st) {
+    void* stream = (void*)st;
     MGB_TRY(mgb_match_frequencies(plan, L, dev->d_target_lr, dev->d_result_lr, nullptr, dev->d_workspace, dev->d_state, stream));
     MGB_TRY(mgb_correct_levels(plan, L, dev->d_workspace, dev->d_state, stream));
     void* outs[3] = {h_out_limited, h_out_no_limiter, h_out_normalized};

@@ -32,9 +32,27 @@ struct Workspace {
     unsigned char* lookback;// [nchunks] LookbackSlot
     int64_t limiter_zero_bytes;
     unsigned char* limiter_planes;  // the wide-window limiter's planes (limiter_plane_bytes; none for the halo kernel)
+    const mgb_reference_profile* profile;  // profiled layouts only: the job's copy of the reference profile (else null)
     int64_t design_stride;  // doubles per channel in `design`
     int64_t total_bytes;
 };
+
+// Piece geometry of one signal (match_levels.py:47-59) and its analysis work items.
+struct ReferenceGeometry {
+    int64_t frames, piece;
+    int32_t divisions, slots;
+};
+// mgb_analyze_reference's workspace: the analysis partials of the reference and its loudest-piece mask
+struct ReferenceRegions {
+    float* spec_part;     // [D][S][2][n_lin]
+    double* sumsq_part;   // [D][S]
+    float* absmax_part;   // [D*S + 1]
+    unsigned char* mask;  // [D]
+    int64_t total_bytes;
+};
+inline int64_t reference_profile_bytes(const mgb_plan& plan) {
+    return (int64_t)sizeof(mgb_reference_profile) + 2LL * plan.n_lin * 8;
+}
 
 // One chunk's published scan state: value and status travel in ONE aligned 16-byte word, so a
 // reader gets a consistent pair from a single load (no flag-then-fence-then-value round trips).
@@ -103,6 +121,9 @@ int launch_analyze(const mgb_plan& plan, const float2* x, int64_t frames, int64_
 int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws,
                   const double* avg_override, double* fir_out, mgb_track_state* state, cudaStream_t stream);
 int64_t design_doubles_per_channel(const mgb_plan& plan);
+// the reference's analysis partials (ReferenceRegions) -> a profile blob at `out` (header + spectra)
+int launch_reference_profile(const mgb_plan& plan, const ReferenceGeometry& g, const ReferenceRegions& r,
+                             mgb_reference_profile* out, cudaStream_t stream);
 int64_t operator_workspace_bytes(const mgb_plan& plan);
 int build_operator(const mgb_plan& plan, double* op_out, void* workspace, cudaStream_t stream);
 extern int g_design_direct;  // tests: force the direct (non-operator) smoothing in mgb_test_design_fir

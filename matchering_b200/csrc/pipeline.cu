@@ -139,6 +139,12 @@ int mgb_pipeline_create(const mgb_plan* plan, int64_t max_target_frames, int64_t
         worst.target_slots = (int32_t)((std::max<int64_t>(cap, worst.target_divisions) + worst.target_divisions - 1) / worst.target_divisions);
         worst.reference_slots = (int32_t)((std::max<int64_t>(cap, worst.reference_divisions) + worst.reference_divisions - 1) / worst.reference_divisions);
         p->workspace_bytes = carve_workspace(*plan, worst, nullptr).total_bytes;
+        // a profiled job has the same target regions, no reference regions and a copy of the profile, which
+        // can be larger than a short reference's regions
+        mgb_track_layout profiled = worst;
+        profiled.reference_frames = profiled.reference_piece = 0;
+        profiled.reference_divisions = profiled.reference_slots = 0;
+        p->workspace_bytes = std::max(p->workspace_bytes, carve_workspace(*plan, profiled, nullptr).total_bytes);
     }
     p->slots.resize(depth);
 #ifndef MGB_EMULATE
@@ -221,9 +227,15 @@ int mgb_pipeline_wait(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out)
     return MGB_OK;
 }
 
-int mgb_pipeline_submit(mgb_pipeline* p, const float* h_target_lr, int64_t target_frames, const float* h_reference_lr,
-                        int64_t reference_frames, float* h_out_limited, int32_t* slot_out) {
-    MGB_REQUIRE(p && h_target_lr && h_reference_lr && h_out_limited, MGB_ERR_INVALID, "pipeline: NULL argument");
+// Stage 1 of a submission: the reference's samples (d_profile == nullptr) or a profile.
+static int submit_levels(mgb_pipeline* p, Slot& s, const void* d_profile, void* sc) {
+    if (d_profile) return mgb_match_levels_profiled(&p->plan, &s.layout, s.d_target, d_profile, s.d_workspace, s.d_state, sc);
+    return mgb_match_levels(&p->plan, &s.layout, s.d_target, s.d_reference, s.d_workspace, s.d_state, sc);
+}
+
+static int submit_impl(mgb_pipeline* p, const float* h_target_lr, int64_t target_frames, const float* h_reference_lr,
+                       int64_t reference_frames, const void* d_profile, float* h_out_limited, int32_t* slot_out) {
+    MGB_REQUIRE(p && h_target_lr && (h_reference_lr || d_profile) && h_out_limited, MGB_ERR_INVALID, "pipeline: NULL argument");
     MGB_REQUIRE(target_frames <= p->max_target && reference_frames <= p->max_reference, MGB_ERR_INVALID,
                 "pipeline: track longer than the pipeline was created for");
     const int idx = p->next;
@@ -231,21 +243,24 @@ int mgb_pipeline_submit(mgb_pipeline* p, const float* h_target_lr, int64_t targe
     Slot& s = p->slots[idx];
     MGB_TRY(mgb_pipeline_wait(p, idx, nullptr));  // the slot's previous result must have left the device
     SubmitGuard guard{p, &s};
-    MGB_TRY(mgb_track_layout_init(&p->plan, target_frames, reference_frames, &s.layout));
+    if (d_profile)
+        MGB_TRY(mgb_track_layout_init_profiled(&p->plan, target_frames, &s.layout));
+    else
+        MGB_TRY(mgb_track_layout_init(&p->plan, target_frames, reference_frames, &s.layout));
     MGB_REQUIRE(s.layout.workspace_bytes <= p->workspace_bytes, MGB_ERR_WORKSPACE, "pipeline: workspace too small");
     const size_t tb = (size_t)target_frames * 8, rb = (size_t)reference_frames * 8;
 #ifdef MGB_EMULATE
     memcpy(s.d_target, h_target_lr, tb);
-    memcpy(s.d_reference, h_reference_lr, rb);
+    if (!d_profile) memcpy(s.d_reference, h_reference_lr, rb);
     void* sc = nullptr;
 #else
     MGB_CUDA_OK(cudaMemcpyAsync(s.d_target, h_target_lr, tb, cudaMemcpyHostToDevice, p->s_h2d));
-    MGB_CUDA_OK(cudaMemcpyAsync(s.d_reference, h_reference_lr, rb, cudaMemcpyHostToDevice, p->s_h2d));
+    if (!d_profile) MGB_CUDA_OK(cudaMemcpyAsync(s.d_reference, h_reference_lr, rb, cudaMemcpyHostToDevice, p->s_h2d));
     MGB_CUDA_OK(cudaEventRecord(s.h2d_done, p->s_h2d));
     MGB_CUDA_OK(cudaStreamWaitEvent(s.compute, s.h2d_done, 0));
     void* sc = (void*)s.compute;
 #endif
-    MGB_TRY(mgb_match_levels(&p->plan, &s.layout, s.d_target, s.d_reference, s.d_workspace, s.d_state, sc));
+    MGB_TRY(submit_levels(p, s, d_profile, sc));
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
@@ -265,11 +280,23 @@ int mgb_pipeline_submit(mgb_pipeline* p, const float* h_target_lr, int64_t targe
     return MGB_OK;
 }
 
-int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
-                            const void* h_reference_pcm, int32_t reference_bits, int64_t reference_frames,
-                            void* h_out_pcm, int32_t out_bits, int32_t* slot_out) {
-    MGB_REQUIRE(p && h_target_pcm && h_reference_pcm && h_out_pcm, MGB_ERR_INVALID, "pipeline: NULL argument");
-    MGB_REQUIRE((target_bits == 16 || target_bits == 24) && (reference_bits == 16 || reference_bits == 24) &&
+int mgb_pipeline_submit(mgb_pipeline* p, const float* h_target_lr, int64_t target_frames, const float* h_reference_lr,
+                        int64_t reference_frames, float* h_out_limited, int32_t* slot_out) {
+    MGB_REQUIRE(h_reference_lr, MGB_ERR_INVALID, "pipeline: NULL argument");
+    return submit_impl(p, h_target_lr, target_frames, h_reference_lr, reference_frames, nullptr, h_out_limited, slot_out);
+}
+
+int mgb_pipeline_submit_profiled(mgb_pipeline* p, const float* h_target_lr, int64_t target_frames, const void* d_profile,
+                                 float* h_out_limited, int32_t* slot_out) {
+    MGB_REQUIRE(d_profile, MGB_ERR_INVALID, "pipeline: NULL argument");
+    return submit_impl(p, h_target_lr, target_frames, nullptr, 0, d_profile, h_out_limited, slot_out);
+}
+
+static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
+                           const void* h_reference_pcm, int32_t reference_bits, int64_t reference_frames, const void* d_profile,
+                           void* h_out_pcm, int32_t out_bits, int32_t* slot_out) {
+    MGB_REQUIRE(p && h_target_pcm && (h_reference_pcm || d_profile) && h_out_pcm, MGB_ERR_INVALID, "pipeline: NULL argument");
+    MGB_REQUIRE((target_bits == 16 || target_bits == 24) && (d_profile || reference_bits == 16 || reference_bits == 24) &&
                     (out_bits == 16 || out_bits == 24),
                 MGB_ERR_UNSUPPORTED, "pipeline: PCM widths must be 16 or 24 bits");
     MGB_REQUIRE(target_frames <= p->max_target && reference_frames <= p->max_reference, MGB_ERR_INVALID,
@@ -279,7 +306,10 @@ int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t t
     Slot& s = p->slots[idx];
     MGB_TRY(mgb_pipeline_wait(p, idx, nullptr));
     SubmitGuard guard{p, &s};
-    MGB_TRY(mgb_track_layout_init(&p->plan, target_frames, reference_frames, &s.layout));
+    if (d_profile)
+        MGB_TRY(mgb_track_layout_init_profiled(&p->plan, target_frames, &s.layout));
+    else
+        MGB_TRY(mgb_track_layout_init(&p->plan, target_frames, reference_frames, &s.layout));
     MGB_REQUIRE(s.layout.workspace_bytes <= p->workspace_bytes, MGB_ERR_WORKSPACE, "pipeline: workspace too small");
     const size_t tb = (size_t)target_frames * 2 * (target_bits / 8), rb = (size_t)reference_frames * 2 * (reference_bits / 8);
     const size_t ob = (size_t)target_frames * 2 * (out_bits / 8);
@@ -287,18 +317,18 @@ int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t t
     unsigned char* pcm_r = pcm_t + (tb + 255) / 256 * 256;
 #ifdef MGB_EMULATE
     memcpy(pcm_t, h_target_pcm, tb);
-    memcpy(pcm_r, h_reference_pcm, rb);
+    if (!d_profile) memcpy(pcm_r, h_reference_pcm, rb);
     void* sc = nullptr;
 #else
     MGB_CUDA_OK(cudaMemcpyAsync(pcm_t, h_target_pcm, tb, cudaMemcpyHostToDevice, p->s_h2d));
-    MGB_CUDA_OK(cudaMemcpyAsync(pcm_r, h_reference_pcm, rb, cudaMemcpyHostToDevice, p->s_h2d));
+    if (!d_profile) MGB_CUDA_OK(cudaMemcpyAsync(pcm_r, h_reference_pcm, rb, cudaMemcpyHostToDevice, p->s_h2d));
     MGB_CUDA_OK(cudaEventRecord(s.h2d_done, p->s_h2d));
     MGB_CUDA_OK(cudaStreamWaitEvent(s.compute, s.h2d_done, 0));
     void* sc = (void*)s.compute;
 #endif
     MGB_TRY(mgb_pcm_decode(pcm_t, target_bits, s.d_target, target_frames * 2, sc));
-    MGB_TRY(mgb_pcm_decode(pcm_r, reference_bits, s.d_reference, reference_frames * 2, sc));
-    MGB_TRY(mgb_match_levels(&p->plan, &s.layout, s.d_target, s.d_reference, s.d_workspace, s.d_state, sc));
+    if (!d_profile) MGB_TRY(mgb_pcm_decode(pcm_r, reference_bits, s.d_reference, reference_frames * 2, sc));
+    MGB_TRY(submit_levels(p, s, d_profile, sc));
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
@@ -317,6 +347,21 @@ int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t t
     guard.ok = true;
     if (slot_out) *slot_out = idx;
     return MGB_OK;
+}
+
+int mgb_pipeline_submit_pcm(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
+                            const void* h_reference_pcm, int32_t reference_bits, int64_t reference_frames,
+                            void* h_out_pcm, int32_t out_bits, int32_t* slot_out) {
+    MGB_REQUIRE(h_reference_pcm, MGB_ERR_INVALID, "pipeline: NULL argument");
+    return submit_pcm_impl(p, h_target_pcm, target_bits, target_frames, h_reference_pcm, reference_bits, reference_frames,
+                           nullptr, h_out_pcm, out_bits, slot_out);
+}
+
+int mgb_pipeline_submit_pcm_profiled(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
+                                     const void* d_profile, void* h_out_pcm, int32_t out_bits, int32_t* slot_out) {
+    MGB_REQUIRE(d_profile, MGB_ERR_INVALID, "pipeline: NULL argument");
+    return submit_pcm_impl(p, h_target_pcm, target_bits, target_frames, nullptr, 16, 0, d_profile, h_out_pcm, out_bits,
+                           slot_out);
 }
 
 int mgb_pipeline_streams(mgb_pipeline* p, void** h2d, void** compute, void** d2h) {

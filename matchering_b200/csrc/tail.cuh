@@ -43,6 +43,43 @@ __device__ __forceinline__ float warp_max_f(float v) {
     return v;
 }
 
+// normalize_reference's coefficient from the reference's peak (dsp.py:96-99)
+__device__ __forceinline__ double reference_coef(double peak, double threshold, double eps) {
+    double coef = 1.0;
+    if (peak < threshold) coef = fmax(eps, peak / threshold);
+    return coef;
+}
+
+// One signal's half of the level statistics (match_levels.py:62-71): the match RMS over its loud pieces and their
+// number.  All 32 lanes of ONE warp call; if `mask` is not null the warp writes the signal's loudest-piece mask there.
+struct SignalLevels {
+    double match;
+    int loud;
+};
+__device__ __forceinline__ SignalLevels signal_levels_warp(const double* part, int div, int slots, double piece,
+                                                           unsigned char* mask) {
+    const int lane = threadIdx.x & 31;
+    double acc = 0.0;
+    for (int p = lane; p < div; p += 32) {
+        const double r = piece_rms(part, p, slots, piece);
+        acc += r * r;
+    }
+    const double avg = sqrt(warp_sum(acc) / (double)div);  // rms(rmses), match_levels.py:101
+    double accm = 0.0, cnt = 0.0;
+    for (int p = lane; p < div; p += 32) {
+        const double r = piece_rms(part, p, slots, piece);
+        const bool m = r >= avg;  // match_levels.py:65
+        if (mask) mask[p] = m ? 1 : 0;
+        if (m) {
+            accm += r * r;
+            cnt += 1.0;
+        }
+    }
+    const double tm = warp_sum(accm);
+    const double tc = warp_sum(cnt);
+    return SignalLevels{sqrt(tm / tc), (int)tc};
+}
+
 // All 32 lanes of ONE warp call (no block barrier inside); every lane gets the result.  If `mask_t` /
 // `mask_r` (shared or global, [div_t] / [div_r]) are not null the warp writes the loudest-piece masks there.
 __device__ __forceinline__ LevelsResult levels_compute_warp(const LevelsArgs& a, unsigned char* mask_t, unsigned char* mask_r) {
@@ -52,43 +89,14 @@ __device__ __forceinline__ LevelsResult levels_compute_warp(const LevelsArgs& a,
     const int peaks = a.div_r_items_override > 0 ? a.div_r_items_override : a.div_r * a.slots_r + 1;
     for (int i = lane; i < peaks; i += 32) pk = fmaxf(pk, a.absmax_r[i]);
     out.peak = (double)warp_max_f(pk);
-    out.coef = 1.0;
-    if (out.peak < a.threshold) out.coef = fmax(a.eps, out.peak / a.threshold);  // dsp.py:96-99
-
-    double match[2];
-    int loud[2];
-    for (int sig = 0; sig < 2; ++sig) {
-        const double* part = sig == 0 ? a.sumsq_t : a.sumsq_r;
-        const int div = sig == 0 ? a.div_t : a.div_r;
-        const int slots = sig == 0 ? a.slots_t : a.slots_r;
-        const double piece = (double)(sig == 0 ? a.piece_t : a.piece_r);
-        unsigned char* mask = sig == 0 ? mask_t : mask_r;
-        double acc = 0.0;
-        for (int p = lane; p < div; p += 32) {
-            const double r = piece_rms(part, p, slots, piece);
-            acc += r * r;
-        }
-        const double avg = sqrt(warp_sum(acc) / (double)div);  // rms(rmses), match_levels.py:101
-        double accm = 0.0, cnt = 0.0;
-        for (int p = lane; p < div; p += 32) {
-            const double r = piece_rms(part, p, slots, piece);
-            const bool m = r >= avg;  // match_levels.py:65
-            if (mask) mask[p] = m ? 1 : 0;
-            if (m) {
-                accm += r * r;
-                cnt += 1.0;
-            }
-        }
-        const double tm = warp_sum(accm);
-        const double tc = warp_sum(cnt);
-        match[sig] = sqrt(tm / tc);
-        loud[sig] = (int)tc;
-    }
-    out.match_t = match[0];
-    out.match_r = match[1] / out.coef;  // the reference measures the normalised reference
+    out.coef = reference_coef(out.peak, a.threshold, a.eps);
+    const SignalLevels t = signal_levels_warp(a.sumsq_t, a.div_t, a.slots_t, (double)a.piece_t, mask_t);
+    const SignalLevels r = signal_levels_warp(a.sumsq_r, a.div_r, a.slots_r, (double)a.piece_r, mask_r);
+    out.match_t = t.match;
+    out.match_r = r.match / out.coef;  // the reference measures the normalised reference
     out.c0 = out.match_r / fmax(a.eps, out.match_t);
-    out.loud_t = loud[0];
-    out.loud_r = loud[1];
+    out.loud_t = t.loud;
+    out.loud_r = r.loud;
     return out;
 }
 

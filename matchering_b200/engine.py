@@ -78,6 +78,12 @@ class DevicePlan:
                                                               reference_frames, C.byref(L)))
         return L
 
+    def layout_profiled(self, target_frames: int) -> _native.TrackLayout:
+        """Layout of a job whose reference comes from a ReferenceProfile (no reference pieces)."""
+        L = _native.TrackLayout()
+        _native.check(self.lib, self.lib.mgb_track_layout_init_profiled(C.byref(self.struct), target_frames, C.byref(L)))
+        return L
+
 
 def limiter_params(lc: _plan.LimiterConstants) -> _native.LimiterParams:
     return _native.LimiterParams.from_constants(lc)
@@ -128,13 +134,15 @@ def to_host_like(t: torch.Tensor, like):
 
 
 class TrackSession:
-    """Buffers for one (plan, target length, reference length) and the stage calls over them."""
+    """Buffers for one (plan, target length, reference length) and the stage calls over them;
+    reference_frames None: the reference comes from a profile (match_levels_profiled)."""
 
-    def __init__(self, plan: DevicePlan, target_frames: int, reference_frames: int):
+    def __init__(self, plan: DevicePlan, target_frames: int, reference_frames: int | None):
         self.plan = plan
         self.lib = plan.lib
         self.device = plan.device
-        self.layout = plan.layout(target_frames, reference_frames)
+        self.layout = (plan.layout_profiled(target_frames) if reference_frames is None
+                       else plan.layout(target_frames, reference_frames))
         self.workspace = torch.empty(int(self.layout.workspace_bytes), dtype=torch.uint8, device=self.device)
         self.state = torch.zeros(C.sizeof(_native.TrackState), dtype=torch.uint8, device=self.device)
         self.result = torch.empty((target_frames, 2), dtype=torch.float32, device=self.device)
@@ -148,6 +156,12 @@ class TrackSession:
         _native.check(self.lib, self.lib.mgb_match_levels(p, l, target.data_ptr(), reference.data_ptr(),
                                                          self.workspace.data_ptr(), self.state.data_ptr(),
                                                          _stream_ptr(self.device)))
+
+    def match_levels_profiled(self, target: torch.Tensor, d_profile: torch.Tensor) -> None:
+        p, l = self._args()
+        _native.check(self.lib, self.lib.mgb_match_levels_profiled(p, l, target.data_ptr(), d_profile.data_ptr(),
+                                                                  self.workspace.data_ptr(), self.state.data_ptr(),
+                                                                  _stream_ptr(self.device)))
 
     def match_frequencies(self, target: torch.Tensor, fir_out: torch.Tensor | None = None) -> None:
         p, l = self._args()
@@ -297,11 +311,13 @@ def host_session(plan: DevicePlan, target_frames: int, reference_frames: int) ->
         sess = TrackSession(plan, target_frames, reference_frames)
         dev = plan.device
         sess.d_target = torch.empty((target_frames, 2), dtype=torch.float32, device=dev)
-        sess.d_reference = torch.empty((reference_frames, 2), dtype=torch.float32, device=dev)
+        sess.d_reference = (None if reference_frames is None
+                            else torch.empty((reference_frames, 2), dtype=torch.float32, device=dev))
         sess.d_out = torch.empty((target_frames, 2), dtype=torch.float32, device=dev)
         sess.d_wide = torch.empty((target_frames, 2), dtype=torch.float64, device=dev)
         b = _native.HostBuffers()
-        b.d_target_lr, b.d_reference_lr = sess.d_target.data_ptr(), sess.d_reference.data_ptr()
+        b.d_target_lr = sess.d_target.data_ptr()
+        b.d_reference_lr = sess.d_reference.data_ptr() if sess.d_reference is not None else None
         b.d_result_lr, b.d_out_lr, b.d_wide = sess.result.data_ptr(), sess.d_out.data_ptr(), sess.d_wide.data_ptr()
         b.d_workspace, b.d_state = sess.workspace.data_ptr(), sess.state.data_ptr()
         sess.host_buffers = b
@@ -327,6 +343,27 @@ def stages_main_host(plan: DevicePlan, target: np.ndarray, reference: np.ndarray
     with io.lock:
         status = io.lib.mgb_stages_main_host(
             io.handle, C.byref(plan.struct), C.byref(sess.layout), target.ctypes.data, reference.ctypes.data, width,
+            ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), width, C.byref(sess.host_buffers), C.byref(state),
+            _stream_ptr(plan.device))
+    _native.check(io.lib, status)
+    return tuple(outs), state
+
+
+def stages_main_host_profiled(plan: DevicePlan, target: np.ndarray, profile, need_default: bool, need_no_limiter: bool,
+                              need_no_limiter_normalized: bool):
+    """stages_main_host with the reference from a ReferenceProfile (mgb_stages_main_host_profiled): only the
+    target is uploaded.  -> ((limited, plain, normalized), TrackState)"""
+    io = HostIO.get()
+    d_profile = profile.checked_blob(plan)
+    sess = host_session(plan, target.shape[0], None)
+    width = target.dtype.itemsize
+    outs = [io.pool.array(target.shape, target.dtype) if need else None
+            for need in (need_default, need_no_limiter, need_no_limiter_normalized)]
+    state = _native.TrackState()
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    with io.lock:
+        status = io.lib.mgb_stages_main_host_profiled(
+            io.handle, C.byref(plan.struct), C.byref(sess.layout), target.ctypes.data, width, d_profile.data_ptr(),
             ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), width, C.byref(sess.host_buffers), C.byref(state),
             _stream_ptr(plan.device))
     _native.check(io.lib, status)

@@ -6,8 +6,10 @@ from __future__ import annotations
 import torch
 
 from .defaults import Config
-from .engine import TrackSession, get_plan, host_array_ok, stages_main_host, to_device_f32, to_host_like
+from .engine import (TrackSession, get_plan, host_array_ok, stages_main_host, stages_main_host_profiled, to_device_f32,
+                     to_host_like)
 from .log import Code, info, debug, debug_line, debug_enabled
+from .profile import ReferenceProfile
 from .utils import to_db
 
 
@@ -16,13 +18,18 @@ def main(target, reference, config: Config, need_default: bool = True, need_no_l
     """target, reference: (N, 2) stereo at config.internal_sample_rate, numpy (float64 like the
     reference's loader produces, or float32) or torch tensors.  Returns
     (result, result_no_limiter, result_no_limiter_normalized), None where not requested, in the
-    caller's array type.
+    caller's array type.  `reference` may also be a ReferenceProfile (profile.analyze_reference): the
+    level statistics and FIR are bit-identical to passing the samples it was made from, and no reference bytes
+    are moved.
 
     numpy in -> the whole job is ONE native call (mgb_stages_main_host): the library narrows and uploads
     the caller's pageable arrays chunk by chunk on its own worker threads, runs the four stages and
     returns float64 (or float32) arrays DMA'd into pooled pinned memory.  torch in -> the staged path
     below, results stay on the device."""
-    if host_array_ok(target) and host_array_ok(reference):
+    profiled = isinstance(reference, ReferenceProfile)
+    if profiled:
+        reference.check_config(config)
+    if host_array_ok(target) and (profiled or host_array_ok(reference)):
         plan = get_plan(config)
         with torch.cuda.device(plan.device):
             debug_line()
@@ -32,19 +39,28 @@ def main(target, reference, config: Config, need_default: bool = True, need_no_l
             info(Code.INFO_MATCHING_FREQS)           # stages.py:117
             info(Code.INFO_CORRECTING_LEVELS)        # stages.py:147
             info(Code.INFO_FINALIZING)               # stages.py:182
-            outs, st = stages_main_host(plan, target, reference, need_default, need_no_limiter,
-                                        need_no_limiter_normalized)
+            if profiled:
+                outs, st = stages_main_host_profiled(plan, target, reference, need_default, need_no_limiter,
+                                                     need_no_limiter_normalized)
+            else:
+                outs, st = stages_main_host(plan, target, reference, need_default, need_no_limiter,
+                                            need_no_limiter_normalized)
             if debug_enabled():
-                _debug_scalars(st, plan.layout(target.shape[0], reference.shape[0]))
+                L = (plan.layout_profiled(target.shape[0]) if profiled
+                     else plan.layout(target.shape[0], reference.shape[0]))
+                _debug_scalars(st, L, reference if profiled else None)
         return outs
     outs = main_device(target, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
     return tuple(None if t is None else to_host_like(t, target) for t in outs)
 
 
-def _debug_scalars(st, L) -> None:
+def _debug_scalars(st, L, profile: ReferenceProfile | None = None) -> None:
     debug(f"The TARGET will be didived into {L.target_divisions} pieces of {L.target_piece} samples; "
           f"{st.target_loud_pieces} of them are at least as loud as the average")
-    debug(f"The REFERENCE will be didived into {L.reference_divisions} pieces of {L.reference_piece} samples; "
+    # a profiled layout has no reference pieces of its own: the profile recorded the reference's geometry
+    divisions, piece = (profile.divisions, profile.piece) if profile is not None else (L.reference_divisions,
+                                                                                        L.reference_piece)
+    debug(f"The REFERENCE will be didived into {divisions} pieces of {piece} samples; "
           f"{st.reference_loud_pieces} of them are at least as loud as the average")
     if st.final_amplitude_coef != 1.0:
         debug(f"The REFERENCE was normalized. Final amplitude coefficient for the TARGET audio is: "
@@ -58,21 +74,31 @@ def _debug_scalars(st, L) -> None:
 def main_device(target, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
                 need_no_limiter_normalized: bool = False):
     """Same as `main`, but the results stay on the device as float32 CUDA tensors (the caller may
-    quantise them there, see core.process)."""
+    quantise them there, see core.process).  `reference` may be a ReferenceProfile."""
+    profiled = isinstance(reference, ReferenceProfile)
+    if profiled:
+        reference.check_config(config)
     plan = get_plan(config)
     device = plan.device
-    if target.ndim != 2 or reference.ndim != 2 or target.shape[1] != 2 or reference.shape[1] != 2:
+    if target.ndim != 2 or target.shape[1] != 2 or (not profiled and (reference.ndim != 2 or reference.shape[1] != 2)):
         raise ValueError("target and reference must be (frames, 2) stereo arrays")
     with torch.cuda.device(device):
         d_target = to_device_f32(target, device)
-        d_reference = to_device_f32(reference, device)
-        session = TrackSession(plan, d_target.shape[0], d_reference.shape[0])
+        if profiled:
+            d_profile = reference.checked_blob(plan)
+            session = TrackSession(plan, d_target.shape[0], None)
+        else:
+            d_reference = to_device_f32(reference, device)
+            session = TrackSession(plan, d_target.shape[0], d_reference.shape[0])
 
         debug_line()
         info(Code.INFO_MATCHING_LEVELS)          # stages.py:52
         debug(f"The maximum size of the analyzed piece: {config.max_piece_size} samples "
               f"or {config.max_piece_size / config.internal_sample_rate:.2f} seconds")
-        session.match_levels(d_target, d_reference)
+        if profiled:
+            session.match_levels_profiled(d_target, d_profile)
+        else:
+            session.match_levels(d_target, d_reference)
 
         debug_line()
         info(Code.INFO_MATCHING_FREQS)           # stages.py:117
@@ -87,6 +113,6 @@ def main_device(target, reference, config: Config, need_default: bool = True, ne
         limited, plain, normalized = session.finalize(need_default, need_no_limiter, need_no_limiter_normalized)
 
         if debug_enabled():  # one read-back of the device scalars, only when somebody listens
-            _debug_scalars(session.read_state(), session.layout)
+            _debug_scalars(session.read_state(), session.layout, reference if profiled else None)
 
     return limited, plain, normalized

@@ -17,6 +17,21 @@ GROUPS = OrderedDict([
 ])
 sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
 demangle = lambda n: subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip()
+
+
+def without_parameters(name):
+    """Cut the parameter list: the first '(' outside the template brackets (template arguments such as
+    `(MeanMode)1` keep their parentheses, so every instantiation keeps its own row)."""
+    depth = 0
+    for i, ch in enumerate(name):
+        depth += ch == "<"
+        depth -= ch == ">"
+        if ch == "(" and depth == 0:
+            return name[:i]
+    return name
+
+
+
 kernels, current = OrderedDict(), None
 arch = re.search(r"arch = (sm_\w+)", sass)
 for line in sass.splitlines():
@@ -24,7 +39,7 @@ for line in sass.splitlines():
     if m:
         name = demangle(m.group(1))
         name = name.replace("void ", "").replace("mgb::", "").replace("(anonymous namespace)::", "")
-        name = re.sub(r"\(.*", "", name)
+        name = without_parameters(name)
         current = kernels.setdefault(name, Counter())
         continue
     m = re.match(r"\s+/\*[0-9a-f]+\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.]*)", line)
