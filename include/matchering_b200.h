@@ -292,6 +292,50 @@ int64_t mgb_limiter_workspace_bytes(const mgb_limiter_params* params, int64_t fr
 int mgb_limit(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,
               void* d_workspace, int64_t workspace_bytes, int32_t* d_engaged, void* stream);
 
+/* ---- loudness meter: ITU-R BS.1770-4 / EBU R 128 ---------------------------------------------
+ * Integrated loudness (gated), loudness range (EBU Tech 3342), maximum momentary and short-term loudness,
+ * sample peak and true peak of `frames` interleaved stereo float32 frames, both channels weighted 1.
+ * K-weighting = the shelf section, then the high-pass section, each an order-2 recursive filter started from rest
+ * (scipy.signal.lfilter), run in float64.  Sub-blocks of `block` = (sample_rate + 5) / 10 frames; momentary =
+ * 4 sub-blocks, short-term = 30, complete windows only.  True peak = max |upfirdn(tp_taps, x_channel, up=oversample)|.
+ * matchering_b200/plan.py (loudness_constants) derives every field below from the sample rate. */
+#define MGB_LOUDNESS_MAX_TAPS 49 /* 12 * oversample + 1 at oversample 4 */
+typedef struct mgb_loudness_params {
+    int32_t sample_rate;      /* 8000 .. 384000 */
+    int32_t block;            /* sub-block length in frames: (sample_rate + 5) / 10 */
+    int32_t oversample;       /* true-peak oversampling: 4 below 96 kHz, 2 below 192 kHz, else 1 */
+    int32_t taps;             /* 12 * oversample + 1 */
+    double shelf_b[3], shelf_a[3];       /* K-weighting stage 1 (a[0] = 1) */
+    double highpass_b[3], highpass_a[3]; /* K-weighting stage 2 (a[0] = 1) */
+    double tp_taps[MGB_LOUDNESS_MAX_TAPS]; /* true-peak interpolator, `taps` used */
+    const void* d_tables;     /* mgb_loudness_tables_bytes() of device memory filled by mgb_loudness_fill_tables */
+} mgb_loudness_params;
+
+/* Written to device memory by mgb_loudness.  Loudness in LUFS, range in LU: -inf where undefined (no complete
+ * window, or every window gated out); loudness_range 0 when no short-term window survives its gates.  Peaks are
+ * linear (max |x| and max |interpolated x| per channel). */
+typedef struct mgb_loudness_result {
+    double integrated;
+    double loudness_range;
+    double momentary_max;
+    double short_term_max;
+    double sample_peak[2];
+    double true_peak[2];
+    int64_t momentary_count;   /* complete 400 ms windows: max(0, sub-blocks - 3) */
+    int64_t short_term_count;  /* complete 3 s windows: max(0, sub-blocks - 29) */
+} mgb_loudness_result;
+
+/* device bytes of the rate's filter tables (powers of the sections' companion matrices) */
+int64_t mgb_loudness_tables_bytes(void);
+/* builds the tables on the host and copies them to d_tables on `stream` (staged before the call returns) */
+int mgb_loudness_fill_tables(const mgb_loudness_params* params, void* d_tables, void* stream);
+int64_t mgb_loudness_workspace_bytes(const mgb_loudness_params* params, int64_t frames);
+/* Meters d_lr into *d_result (device).  Asynchronous on `stream`; the workspace needs no initialisation.
+ * MGB_ERR_INVALID for a rate outside [8000, 384000], fields that do not follow from the rate, no frames, a
+ * pointer that is not 16-byte aligned or a workspace smaller than mgb_loudness_workspace_bytes. */
+int mgb_loudness(const mgb_loudness_params* params, const float* d_lr, int64_t frames, void* d_workspace,
+                 int64_t workspace_bytes, mgb_loudness_result* d_result, void* stream);
+
 /* ---- whole job with HOST buffers (the call the end-to-end benchmark times) --------------------
  * h_* are host pointers (pinned for full speed).  Copies target and reference to the device,
  * runs stages 1-4 and copies the requested outputs back; synchronises `stream` before returning.
@@ -389,6 +433,14 @@ int mgb_pipeline_submit_profiled(mgb_pipeline* p, const float* h_target_lr, int6
 int mgb_pipeline_submit_pcm_profiled(mgb_pipeline* p, const void* h_target_pcm, int32_t target_bits, int64_t target_frames,
                                      const void* d_profile, void* h_out_pcm, int32_t out_bits, int32_t* slot_out);
 int mgb_pipeline_wait(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out);
+/* Meter every later submission: called before the first submit, it allocates each slot's meter workspace and
+ * result.  Every submit then runs mgb_loudness on its float32 limited output (before any PCM quantisation) on
+ * the slot's compute stream and copies the result back with the state.  params->d_tables must stay valid until
+ * the pipeline is destroyed.  A pipeline that never calls this allocates and launches nothing for metering. */
+int mgb_pipeline_enable_loudness(mgb_pipeline* p, const mgb_loudness_params* params);
+/* mgb_pipeline_wait, and the slot's meter (MGB_ERR_INVALID when metering is not enabled) */
+int mgb_pipeline_wait_loudness(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out,
+                               mgb_loudness_result* loudness_out);
 int mgb_pipeline_streams(mgb_pipeline* p, void** h2d, void** compute, void** d2h);
 int mgb_pipeline_destroy(mgb_pipeline* p);
 

@@ -134,6 +134,39 @@ class ReferenceProfileHeader(C.Structure):
     ]
 
 
+MGB_LOUDNESS_MAX_TAPS = 49
+
+
+class LoudnessParams(C.Structure):
+    _fields_ = [
+        ("sample_rate", C.c_int32), ("block", C.c_int32), ("oversample", C.c_int32), ("taps", C.c_int32),
+        ("shelf_b", C.c_double * 3), ("shelf_a", C.c_double * 3),
+        ("highpass_b", C.c_double * 3), ("highpass_a", C.c_double * 3),
+        ("tp_taps", C.c_double * MGB_LOUDNESS_MAX_TAPS),
+        ("d_tables", C.c_void_p),
+    ]
+
+    @classmethod
+    def from_constants(cls, lc) -> "LoudnessParams":
+        """plan.LoudnessConstants -> the C struct (d_tables left NULL)."""
+        p = cls()
+        p.sample_rate, p.block, p.oversample, p.taps = lc.sample_rate, lc.block, lc.oversample, len(lc.tp_taps)
+        for name in ("shelf_b", "shelf_a", "highpass_b", "highpass_a", "tp_taps"):
+            dst = getattr(p, name)
+            for i, v in enumerate(getattr(lc, name)):
+                dst[i] = float(v)
+        return p
+
+
+class LoudnessResult(C.Structure):
+    _fields_ = [
+        ("integrated", C.c_double), ("loudness_range", C.c_double),
+        ("momentary_max", C.c_double), ("short_term_max", C.c_double),
+        ("sample_peak", C.c_double * 2), ("true_peak", C.c_double * 2),
+        ("momentary_count", C.c_int64), ("short_term_count", C.c_int64),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/matchering_b200.h declares
 PROTOTYPES = {
     "mgb_version": (C.c_int, []),
@@ -195,6 +228,13 @@ PROTOTYPES = {
     "mgb_pipeline_submit_pcm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int32, C.c_int64,
                                           C.c_void_p, C.c_int32, C.POINTER(C.c_int32)]),
     "mgb_pipeline_wait": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TrackState)]),
+    "mgb_pipeline_enable_loudness": (C.c_int, [C.c_void_p, C.POINTER(LoudnessParams)]),
+    "mgb_pipeline_wait_loudness": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TrackState), C.POINTER(LoudnessResult)]),
+    "mgb_loudness_tables_bytes": (C.c_int64, []),
+    "mgb_loudness_fill_tables": (C.c_int, [C.POINTER(LoudnessParams), C.c_void_p, C.c_void_p]),
+    "mgb_loudness_workspace_bytes": (C.c_int64, [C.POINTER(LoudnessParams), C.c_int64]),
+    "mgb_loudness": (C.c_int, [C.POINTER(LoudnessParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                               C.c_void_p]),
     "mgb_pipeline_streams": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
     "mgb_pipeline_destroy": (C.c_int, [C.c_void_p]),
     "mgb_convert_f64_to_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),

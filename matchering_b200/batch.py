@@ -15,23 +15,34 @@ import torch
 
 from . import _native
 from .engine import get_plan
+from .loudness import Loudness, device_meter
 from .profile import ReferenceProfile
 
 
 class MasteringPipeline:
-    def __init__(self, config, max_target_frames: int, max_reference_frames: int, depth: int = 3, device=None):
+    def __init__(self, config, max_target_frames: int, max_reference_frames: int, depth: int = 3, device=None,
+                 loudness: bool = False):
         """max_reference_frames bounds the references submitted as samples; profiles have no such bound
-        (a pipeline that only takes profiles may pass smallest_reference_frames(config))."""
+        (a pipeline that only takes profiles may pass smallest_reference_frames(config)).
+        loudness=True meters every limited output on the device (mg.loudness's meter, at the Config's rate)
+        and `wait_loudness` returns it."""
         self.config = config
         self.plan = get_plan(config, device)
         self.lib = self.plan.lib
         self.device = self.plan.device
         self.depth = depth
         self._handle = C.c_void_p()
+        # (the meter's tables are cached per device and rate: they outlive the pipeline)
+        self._meter = device_meter(config.internal_sample_rate, self.device) if loudness else None
+        self._pending = {}  # slot -> (target, reference, out) kept alive until the slot is waited on
         with torch.cuda.device(self.device):
             _native.check(self.lib, self.lib.mgb_pipeline_create(C.byref(self.plan.struct), max_target_frames,
                                                                  max_reference_frames, depth, C.byref(self._handle)))
-        self._pending = {}  # slot -> (target, reference, out) kept alive until the slot is waited on
+            if loudness:
+                status = self.lib.mgb_pipeline_enable_loudness(self._handle, C.byref(self._meter.params))
+                if status != _native.MGB_OK:
+                    self.close()
+                    _native.check(self.lib, status)
 
     @staticmethod
     def _ptr(a):
@@ -104,6 +115,15 @@ class MasteringPipeline:
         self._pending.pop(slot, None)
         return st
 
+    def wait_loudness(self, slot: int) -> tuple:
+        """wait(slot), and the meter of the slot's limited output: (TrackState, Loudness).  Needs loudness=True."""
+        if self._meter is None:
+            raise ValueError("this pipeline was created without loudness=True")
+        st, res = _native.TrackState(), _native.LoudnessResult()
+        _native.check(self.lib, self.lib.mgb_pipeline_wait_loudness(self._handle, slot, C.byref(st), C.byref(res)))
+        self._pending.pop(slot, None)
+        return st, Loudness.from_result(res)
+
     def wait_all(self) -> None:
         for slot in list(self._pending):
             self.wait(slot)
@@ -131,22 +151,31 @@ def smallest_reference_frames(config) -> int:
     return int(config.fft_size) + 1
 
 
-def master_many(pairs, config, depth: int = 3):
+def master_many(pairs, config, depth: int = 3, loudness: bool = False):
     """[(target, reference), ...] float32 host arrays -> list of limited results (numpy float32).  A reference
-    may be a ReferenceProfile (an album against one reference: analysed once, never copied again)."""
+    may be a ReferenceProfile (an album against one reference: analysed once, never copied again).
+    loudness=True returns (results, meters): each result's Loudness, metered on the device."""
     pairs = list(pairs)
     if not pairs:
-        return []
+        return ([], []) if loudness else []
     for _, r in pairs:  # a Config the profile was not made for fails before any device work
         if isinstance(r, ReferenceProfile):
             r.check_config(config)
     max_t = max(len(t) for t, _ in pairs)
     max_r = max((len(r) for _, r in pairs if not isinstance(r, ReferenceProfile)), default=smallest_reference_frames(config))
     outs = [np.empty((len(t), 2), dtype=np.float32) for t, _ in pairs]
-    with MasteringPipeline(config, max_t, max_r, depth) as pipe:
-        for (t, r), o in zip(pairs, outs):
+    meters = [None] * len(pairs)
+    with MasteringPipeline(config, max_t, max_r, depth, loudness=loudness) as pipe:
+        in_flight = []  # (slot, track) in submission order; slots are reused round-robin
+        for i, ((t, r), o) in enumerate(zip(pairs, outs)):
             if not isinstance(r, ReferenceProfile):
                 r = np.ascontiguousarray(r, dtype=np.float32)
-            pipe.submit(np.ascontiguousarray(t, dtype=np.float32), r, o)
+            if loudness and len(in_flight) == depth:  # collect the meter of the slot this submit reuses
+                slot, k = in_flight.pop(0)
+                meters[k] = pipe.wait_loudness(slot)[1]
+            in_flight.append((pipe.submit(np.ascontiguousarray(t, dtype=np.float32), r, o), i))
+        if loudness:
+            for slot, k in in_flight:
+                meters[k] = pipe.wait_loudness(slot)[1]
         pipe.wait_all()
-    return outs
+    return (outs, meters) if loudness else outs

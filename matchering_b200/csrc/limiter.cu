@@ -801,3 +801,5 @@ int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, doubl
 }
 
 }  // namespace mgb
+
+#include "loudness.cuh"  // the loudness meter: the same scans, look-back words and section tables

@@ -25,6 +25,9 @@ struct Slot {
     void* d_pcm_out = nullptr;  // quantised result
     mgb_track_state* d_state = nullptr;
     mgb_track_state* h_state = nullptr;  // pinned
+    void* d_meter_ws = nullptr;          // metering only (mgb_pipeline_enable_loudness)
+    mgb_loudness_result* d_meter = nullptr;
+    mgb_loudness_result* h_meter = nullptr;  // pinned
     mgb_track_layout layout;
     bool busy = false;
 #ifndef MGB_EMULATE
@@ -42,6 +45,10 @@ struct mgb_pipeline {
     int64_t workspace_bytes = 0;
     std::vector<mgb::Slot> slots;
     int next = 0;
+    bool submitted = false;
+    bool meter = false;  // mgb_pipeline_enable_loudness
+    mgb_loudness_params meter_params;
+    int64_t meter_ws_bytes = 0;
 #ifndef MGB_EMULATE
     cudaStream_t s_h2d = nullptr, s_compute = nullptr, s_d2h = nullptr;
 #endif
@@ -195,10 +202,14 @@ int mgb_pipeline_destroy(mgb_pipeline* p) {
         dev_free(s.d_pcm_in);
         dev_free(s.d_pcm_out);
         dev_free(s.d_state);
+        if (s.d_meter_ws) dev_free(s.d_meter_ws);
+        if (s.d_meter) dev_free(s.d_meter);
 #ifdef MGB_EMULATE
         free(s.h_state);
+        free(s.h_meter);
 #else
         if (s.h_state) cudaFreeHost(s.h_state);
+        if (s.h_meter) cudaFreeHost(s.h_meter);
         if (s.h2d_done) cudaEventDestroy(s.h2d_done);
         if (s.compute_done) cudaEventDestroy(s.compute_done);
         if (s.d2h_done) cudaEventDestroy(s.d2h_done);
@@ -227,6 +238,45 @@ int mgb_pipeline_wait(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out)
     return MGB_OK;
 }
 
+int mgb_pipeline_enable_loudness(mgb_pipeline* p, const mgb_loudness_params* params) {
+    MGB_REQUIRE(p && params, MGB_ERR_INVALID, "pipeline: NULL argument");
+    MGB_REQUIRE(!p->submitted && !p->meter, MGB_ERR_INVALID, "pipeline: metering is enabled once, before the first submit");
+    MGB_REQUIRE(params->d_tables, MGB_ERR_INVALID, "pipeline: loudness tables missing");
+    const int64_t bytes = mgb_loudness_workspace_bytes(params, std::max<int64_t>(p->max_target, 1));
+    MGB_REQUIRE(bytes > 0, MGB_ERR_INVALID, "pipeline: bad loudness parameters");
+    for (auto& s : p->slots) {
+        s.d_meter_ws = dev_alloc((size_t)bytes);
+        s.d_meter = (mgb_loudness_result*)dev_alloc(sizeof(mgb_loudness_result));
+#ifdef MGB_EMULATE
+        s.h_meter = (mgb_loudness_result*)malloc(sizeof(mgb_loudness_result));
+#else
+        if (cudaMallocHost((void**)&s.h_meter, sizeof(mgb_loudness_result)) != cudaSuccess) s.h_meter = nullptr;
+#endif
+        if (!s.d_meter_ws || !s.d_meter || !s.h_meter) {
+            set_error("pipeline: allocation of the meter buffers failed");
+            return MGB_ERR_CUDA;  // (what was allocated is released by mgb_pipeline_destroy)
+        }
+        memset(s.h_meter, 0, sizeof(mgb_loudness_result));
+    }
+    p->meter_params = *params;
+    p->meter_ws_bytes = bytes;
+    p->meter = true;
+    return MGB_OK;
+}
+
+int mgb_pipeline_wait_loudness(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out, mgb_loudness_result* loudness_out) {
+    MGB_REQUIRE(p && p->meter, MGB_ERR_INVALID, "pipeline: metering is not enabled");
+    MGB_TRY(mgb_pipeline_wait(p, slot, state_out));
+    if (loudness_out) *loudness_out = *p->slots[slot].h_meter;
+    return MGB_OK;
+}
+
+// Metering of a submission's float32 limited output, on the slot's compute stream (nothing without metering).
+static int submit_meter(mgb_pipeline* p, Slot& s, int64_t frames, void* sc) {
+    if (!p->meter) return MGB_OK;
+    return mgb_loudness(&p->meter_params, s.d_out, frames, s.d_meter_ws, p->meter_ws_bytes, s.d_meter, sc);
+}
+
 // Stage 1 of a submission: the reference's samples (d_profile == nullptr) or a profile.
 static int submit_levels(mgb_pipeline* p, Slot& s, const void* d_profile, void* sc) {
     if (d_profile) return mgb_match_levels_profiled(&p->plan, &s.layout, s.d_target, d_profile, s.d_workspace, s.d_state, sc);
@@ -243,6 +293,7 @@ static int submit_impl(mgb_pipeline* p, const float* h_target_lr, int64_t target
     Slot& s = p->slots[idx];
     MGB_TRY(mgb_pipeline_wait(p, idx, nullptr));  // the slot's previous result must have left the device
     SubmitGuard guard{p, &s};
+    p->submitted = true;
     if (d_profile)
         MGB_TRY(mgb_track_layout_init_profiled(&p->plan, target_frames, &s.layout));
     else
@@ -264,14 +315,18 @@ static int submit_impl(mgb_pipeline* p, const float* h_target_lr, int64_t target
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
+    MGB_TRY(submit_meter(p, s, target_frames, sc));
 #ifdef MGB_EMULATE
     memcpy(h_out_limited, s.d_out, tb);
     memcpy(s.h_state, s.d_state, sizeof(mgb_track_state));
+    if (p->meter) memcpy(s.h_meter, s.d_meter, sizeof(mgb_loudness_result));
 #else
     MGB_CUDA_OK(cudaEventRecord(s.compute_done, s.compute));
     MGB_CUDA_OK(cudaStreamWaitEvent(p->s_d2h, s.compute_done, 0));
     MGB_CUDA_OK(cudaMemcpyAsync(h_out_limited, s.d_out, tb, cudaMemcpyDeviceToHost, p->s_d2h));
     MGB_CUDA_OK(cudaMemcpyAsync(s.h_state, s.d_state, sizeof(mgb_track_state), cudaMemcpyDeviceToHost, p->s_d2h));
+    if (p->meter)
+        MGB_CUDA_OK(cudaMemcpyAsync(s.h_meter, s.d_meter, sizeof(mgb_loudness_result), cudaMemcpyDeviceToHost, p->s_d2h));
     MGB_CUDA_OK(cudaEventRecord(s.d2h_done, p->s_d2h));
 #endif
     s.busy = true;
@@ -306,6 +361,7 @@ static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t ta
     Slot& s = p->slots[idx];
     MGB_TRY(mgb_pipeline_wait(p, idx, nullptr));
     SubmitGuard guard{p, &s};
+    p->submitted = true;
     if (d_profile)
         MGB_TRY(mgb_track_layout_init_profiled(&p->plan, target_frames, &s.layout));
     else
@@ -332,15 +388,19 @@ static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t ta
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
+    MGB_TRY(submit_meter(p, s, target_frames, sc));  // (the float32 output, before quantisation)
     MGB_TRY(mgb_pcm_encode(s.d_out, out_bits, s.d_pcm_out, target_frames * 2, sc));
 #ifdef MGB_EMULATE
     memcpy(h_out_pcm, s.d_pcm_out, ob);
     memcpy(s.h_state, s.d_state, sizeof(mgb_track_state));
+    if (p->meter) memcpy(s.h_meter, s.d_meter, sizeof(mgb_loudness_result));
 #else
     MGB_CUDA_OK(cudaEventRecord(s.compute_done, s.compute));
     MGB_CUDA_OK(cudaStreamWaitEvent(p->s_d2h, s.compute_done, 0));
     MGB_CUDA_OK(cudaMemcpyAsync(h_out_pcm, s.d_pcm_out, ob, cudaMemcpyDeviceToHost, p->s_d2h));
     MGB_CUDA_OK(cudaMemcpyAsync(s.h_state, s.d_state, sizeof(mgb_track_state), cudaMemcpyDeviceToHost, p->s_d2h));
+    if (p->meter)
+        MGB_CUDA_OK(cudaMemcpyAsync(s.h_meter, s.d_meter, sizeof(mgb_loudness_result), cudaMemcpyDeviceToHost, p->s_d2h));
     MGB_CUDA_OK(cudaEventRecord(s.d2h_done, p->s_d2h));
 #endif
     s.busy = true;

@@ -241,6 +241,51 @@ def limiter_constants(config) -> LimiterConstants:
 
 
 # ------------------------------------------------------------------------------------------------
+# loudness meter constants (ITU-R BS.1770-4), depending on the sample rate only
+# ------------------------------------------------------------------------------------------------
+@dataclass
+class LoudnessConstants:
+    sample_rate: int
+    block: int          # sub-block of 100 ms: (fs + 5) // 10 frames
+    oversample: int     # true-peak oversampling factor
+    shelf_b: np.ndarray
+    shelf_a: np.ndarray
+    highpass_b: np.ndarray
+    highpass_a: np.ndarray
+    tp_taps: np.ndarray  # 12 * oversample + 1 interpolator taps
+
+
+LOUDNESS_MIN_RATE, LOUDNESS_MAX_RATE = 8000, 384000
+
+
+def _k_weighting_section(fs: int, f0: float, q: float):
+    k = math.tan(math.pi * f0 / fs)
+    a0 = 1.0 + k / q + k * k
+    return k, a0, np.array([1.0, 2.0 * (k * k - 1.0) / a0, (1.0 - k / q + k * k) / a0])
+
+
+def loudness_constants(fs: int) -> LoudnessConstants:
+    """K-weighting sections for any rate from their analog prototypes (as libebur128 and pyloudnorm derive them;
+    at 48 kHz they reproduce BS.1770's published coefficients) and the true-peak interpolator."""
+    fs = int(fs)
+    if not LOUDNESS_MIN_RATE <= fs <= LOUDNESS_MAX_RATE:
+        raise ValueError(f"loudness: sample rate {fs} outside [{LOUDNESS_MIN_RATE}, {LOUDNESS_MAX_RATE}]")
+    # high-shelf (the head's acoustic effect)
+    gain_db, f0, q = 3.999843853973347, 1681.974450955533, 0.7071752369554196
+    k, a0, shelf_a = _k_weighting_section(fs, f0, q)
+    vh = 10.0 ** (gain_db / 20.0)
+    vb = vh ** 0.4996667741545416
+    shelf_b = np.array([vh + vb * k / q + k * k, 2.0 * (k * k - vh), vh - vb * k / q + k * k]) / a0
+    # high-pass (RLB weighting)
+    _, _, highpass_a = _k_weighting_section(fs, 38.13547087602444, 0.5003270373238773)
+    highpass_b = np.array([1.0, -2.0, 1.0])
+    os_ = 4 if fs < 96000 else (2 if fs < 192000 else 1)
+    m = np.arange(12 * os_ + 1)
+    taps = np.sinc((m - 6 * os_) / os_) * np.kaiser(12 * os_ + 1, 8.0)
+    return LoudnessConstants(fs, (fs + 5) // 10, os_, shelf_b, shelf_a, highpass_b, highpass_a, taps)
+
+
+# ------------------------------------------------------------------------------------------------
 # the plan
 # ------------------------------------------------------------------------------------------------
 @dataclass
