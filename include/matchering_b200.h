@@ -57,7 +57,11 @@ typedef struct mgb_limiter_params {
                            across chunks instead and needs more workspace (mgb_limiter_workspace_bytes) */
     int32_t hold_order;    /* LimiterConfig.hold_filter_order    (defaults.py:48-50) */
     int32_t release_order; /* LimiterConfig.release_filter_order (defaults.py:54-56) */
-    int32_t reserved;
+    int32_t true_peak;  /* 0: the reference's rectifier max(|L|, |R|).  1, 2 or 4: true-peak mode, the detector's oversampling
+                           factor L (4 below 96 kHz, 2 below 192 kHz, 1 above): the limiter bounds the interpolated
+                           signal, d[n] = max(u[n], u[n-1]) with u the largest |value| of both channels at n + ph/L,
+                           ph = 0 .. L-1, through the meter's interpolator (mgb_true_peak_taps).  Other values:
+                           MGB_ERR_INVALID */
     double attack_c;    /* exp(attack_filter_coefficient / attack_samples) */
     double hold_b[MGB_MAX_FILTER_ORDER + 1], hold_a[MGB_MAX_FILTER_ORDER + 1];       /* butter(order, hold_filter_coefficient, fs) */
     double release_b[MGB_MAX_FILTER_ORDER + 1], release_a[MGB_MAX_FILTER_ORDER + 1]; /* butter(order, release_filter_coefficient/release, fs) */
@@ -287,10 +291,16 @@ int mgb_finalize(const mgb_plan* plan, const mgb_track_layout* layout, const flo
 
 /* ---- limiter.limit (limiter/hyrax.py:78-99), standalone ---------------------------------------
  * d_out = limit(d_in) for `frames` stereo frames.  d_engaged (int32, device) receives 0 when the
- * reference would return its input untouched (hyrax.py:83-85; d_out is then a copy of d_in). */
+ * reference would return its input untouched (hyrax.py:83-85; d_out is then a copy of d_in).  In true-peak mode
+ * (params->true_peak != 0) the early-out and the gain follow the detector d instead of the sample peaks, and the
+ * workspace holds d as well (4 B per frame). */
 int64_t mgb_limiter_workspace_bytes(const mgb_limiter_params* params, int64_t frames);
 int mgb_limit(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,
               void* d_workspace, int64_t workspace_bytes, int32_t* d_engaged, void* stream);
+/* The true-peak mode's interpolator (mgb_limiter_params.true_peak): the 12 * oversample + 1 taps
+ * sinc((m - 6 L)/L) * kaiser(12 L + 1, beta = 8)[m], computed on the host in long double, into out (host memory).
+ * oversample 1, 2 or 4; MGB_ERR_INVALID otherwise.  The same taps as the loudness meter's tp_taps. */
+int mgb_true_peak_taps(int32_t oversample, double* out);
 
 /* ---- loudness meter: ITU-R BS.1770-4 / EBU R 128 ---------------------------------------------
  * Integrated loudness (gated), loudness range (EBU Tech 3342), maximum momentary and short-term loudness,

@@ -30,7 +30,7 @@ class LimiterParams(C.Structure):
         ("warmup", C.c_int32),
         ("hold_order", C.c_int32),
         ("release_order", C.c_int32),
-        ("reserved", C.c_int32),
+        ("true_peak", C.c_int32),
         ("attack_c", C.c_double),
         ("hold_b", C.c_double * (MGB_MAX_FILTER_ORDER + 1)), ("hold_a", C.c_double * (MGB_MAX_FILTER_ORDER + 1)),
         ("release_b", C.c_double * (MGB_MAX_FILTER_ORDER + 1)), ("release_a", C.c_double * (MGB_MAX_FILTER_ORDER + 1)),
@@ -44,6 +44,7 @@ class LimiterParams(C.Structure):
         p.reach, p.hold, p.warmup = lc.reach, lc.hold, lc.warmup
         p.attack_c = lc.attack_c
         p.hold_order, p.release_order = len(lc.hold_a) - 1, len(lc.release_a) - 1
+        p.true_peak = lc.true_peak
         for name in ("hold_b", "hold_a", "release_b", "release_a"):
             dst = getattr(p, name)
             for i, v in enumerate(getattr(lc, name)):
@@ -205,6 +206,7 @@ PROTOTYPES = {
     "mgb_limiter_workspace_bytes": (C.c_int64, [C.POINTER(LimiterParams), C.c_int64]),
     "mgb_limit": (C.c_int, [C.POINTER(LimiterParams), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                             C.c_void_p, C.c_void_p]),
+    "mgb_true_peak_taps": (C.c_int, [C.c_int32, C.c_void_p]),
     "mgb_process_host": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -119,8 +119,11 @@ Workspace carve_workspace(const mgb_plan& plan, const mgb_track_layout& L, void*
     const int64_t limiter_zero_from = off;
     w.tickets = (int*)take(256);
     w.lookback = take(limiter_lookback_bytes(plan.limiter, L.target_frames));
+    const bool tp = plan.limiter.true_peak != 0;  // (true-peak mode only: the detector's maximum and plane)
+    w.tp_peak = tp ? (float*)take(4) : nullptr;
     w.limiter_zero_bytes = off - limiter_zero_from;
     w.limiter_planes = take(limiter_plane_bytes(plan.limiter, L.target_frames));  // (empty unless the wide-window path runs)
+    w.tp_plane = tp ? (float*)take(true_peak_plane_bytes(plan.limiter, L.target_frames)) : nullptr;
     // a profiled layout (no reference pieces): the copy of the profile, behind everything a paired layout has
     w.profile = L.reference_divisions == 0 ? (const mgb_reference_profile*)take(reference_profile_bytes(plan)) : nullptr;
     w.total_bytes = off;
@@ -671,6 +674,22 @@ int mgb_finalize(const mgb_plan* plan, const mgb_track_layout* L, const float* d
     cudaStream_t st = (cudaStream_t)stream;
     Workspace ws = carve_workspace(*plan, *L, d_workspace);
     const float2* res = (const float2*)d_result_lr;
+    const bool tp = plan->limiter.true_peak != 0;
+    auto clear_limiter = [&]() -> int {
+#ifdef MGB_EMULATE
+        memset(ws.tickets, 0, ws.limiter_zero_bytes);
+#else
+        if (cudaMemsetAsync(ws.tickets, 0, ws.limiter_zero_bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+        return MGB_OK;
+    };
+    if (tp && (d_out_limited || d_out_normalized)) {
+        // true-peak mode: the detector over the result, then the normalisation coefficient and the limiter's early-out
+        // from gain * max(d) in place of the sample peak's (correction_final_kernel)
+        MGB_TRY(clear_limiter());
+        MGB_TRY(launch_true_peak_detect(plan->limiter.true_peak, res, L->target_frames, ws.tp_plane, ws.tp_peak, st));
+        MGB_TRY(launch_true_peak_final(ws.tp_peak, plan->min_value, plan->threshold, d_state, st));
+    }
     if (d_out_normalized) {
         MGB_TRY(check_aligned(d_out_normalized, "d_out_normalized"));
         MGB_TRY(launch_scale(res, (float2*)d_out_normalized, L->target_frames, &d_state->gain, &d_state->normalize_coef, st));
@@ -681,31 +700,30 @@ int mgb_finalize(const mgb_plan* plan, const mgb_track_layout* L, const float* d
     }
     if (d_out_limited) {
         MGB_TRY(check_aligned(d_out_limited, "d_out_limited"));
-#ifdef MGB_EMULATE
-        memset(ws.tickets, 0, ws.limiter_zero_bytes);
-#else
-        if (cudaMemsetAsync(ws.tickets, 0, ws.limiter_zero_bytes, st) != cudaSuccess) return cuda_status("memset");
-#endif
+        if (!tp) MGB_TRY(clear_limiter());  // (in true-peak mode, cleared before the detector, which only sets tp_peak)
         MGB_TRY(launch_limiter(plan->limiter, res, (float2*)d_out_limited, L->target_frames, &d_state->gain,
                                &d_state->final_amplitude_coef, &d_state->limiter_engaged, ws.tickets,
-                               ws.lookback, ws.limiter_planes, plan->d_limiter_tables, st));
+                               ws.lookback, ws.limiter_planes, plan->d_limiter_tables, st, false, ws.tp_plane));
     }
     return MGB_OK;
 }
 
-// standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [256, kLimitHeader): pole tables  [kLimitHeader, ...): look-back words,
-// then the wide-window path's planes (none for the halo kernel)
+// standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [32,36): the true-peak detector's maximum  [256, kLimitHeader):
+// pole tables  [kLimitHeader, ...): look-back words, then the wide-window path's planes (none for the halo kernel), then the
+// true-peak detector's plane (true-peak mode only)
 static const int64_t kLimitHeader = 256 + 32768;
 
 int64_t mgb_limiter_workspace_bytes(const mgb_limiter_params* params, int64_t frames) {
     if (!params) return -1;
     if (frames <= 0) return kLimitHeader;
-    return kLimitHeader + limiter_lookback_bytes(*params, frames) + limiter_plane_bytes(*params, frames);
+    return kLimitHeader + limiter_lookback_bytes(*params, frames) + limiter_plane_bytes(*params, frames) +
+           true_peak_plane_bytes(*params, frames);
 }
 
 static int limit_impl(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,
                       void* d_workspace, int64_t workspace_bytes, int32_t* d_engaged, void* stream, bool gains_only) {
     MGB_REQUIRE(params != nullptr, MGB_ERR_INVALID, "params is NULL");
+    MGB_TRY(limiter_validate(*params));
     MGB_TRY(check_aligned(d_in_lr, "d_in_lr"));
     MGB_TRY(check_aligned(d_out_lr, "d_out_lr"));
     MGB_TRY(check_aligned(d_workspace, "d_workspace"));
@@ -727,10 +745,18 @@ static int limit_impl(const mgb_limiter_params* params, const float* d_in_lr, fl
     MGB_TRY(launch_limiter_tables(*params, tables, st));
     float* peak = (float*)base;
     int* ticket = (int*)(base + 16);
-    MGB_TRY(launch_absmax((const float2*)d_in_lr, frames, peak, st));
-    MGB_TRY(launch_limiter_engaged(peak, nullptr, params->threshold, d_engaged, st));
+    float* tp_d = nullptr;
+    if (params->true_peak) {  // the early-out on max(d) instead of the sample peak
+        tp_d = (float*)(base + zero_bytes + limiter_plane_bytes(*params, frames));
+        float* tp_peak = (float*)(base + 32);
+        MGB_TRY(launch_true_peak_detect(params->true_peak, (const float2*)d_in_lr, frames, tp_d, tp_peak, st));
+        MGB_TRY(launch_limiter_engaged(tp_peak, nullptr, params->threshold, d_engaged, st));
+    } else {
+        MGB_TRY(launch_absmax((const float2*)d_in_lr, frames, peak, st));
+        MGB_TRY(launch_limiter_engaged(peak, nullptr, params->threshold, d_engaged, st));
+    }
     return launch_limiter(*params, (const float2*)d_in_lr, (float2*)d_out_lr, frames, nullptr, nullptr, d_engaged, ticket,
-                          base + kLimitHeader, base + zero_bytes, tables, st, gains_only);
+                          base + kLimitHeader, base + zero_bytes, tables, st, gains_only, tp_d);
 }
 
 int mgb_limit(const mgb_limiter_params* params, const float* d_in_lr, float* d_out_lr, int64_t frames,

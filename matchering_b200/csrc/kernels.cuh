@@ -30,8 +30,10 @@ struct Workspace {
     // ---- zeroed before every limiter launch (limiter_zero_bytes from `tickets` on) ----
     int* tickets;           // [64] zeroed counters: 0 = limiter chunk ticket
     unsigned char* lookback;// [nchunks] LookbackSlot
+    float* tp_peak;         // true-peak mode: max(d), float bits (the last word of the zeroed range; else null)
     int64_t limiter_zero_bytes;
-    unsigned char* limiter_planes;  // the wide-window limiter's planes (limiter_plane_bytes; none for the halo kernel)
+    unsigned char* limiter_planes;
+    float* tp_plane;        // true-peak mode: the detector plane d (true_peak_plane_bytes; else null)  // the wide-window limiter's planes (limiter_plane_bytes; none for the halo kernel)
     const mgb_reference_profile* profile;  // profiled layouts only: the job's copy of the reference profile (else null)
     int64_t design_stride;  // doubles per channel in `design`
     int64_t total_bytes;
@@ -154,7 +156,7 @@ int launch_convert_f32_f64(const float* in, double* out, int64_t count, cudaStre
 // (the halo kernel where its span fits, the wide-window path otherwise; wide_planes: limiter_plane_bytes of workspace)
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
                    const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
-                   const void* tables, cudaStream_t stream, bool gains_only = false);
+                   const void* tables, cudaStream_t stream, bool gains_only = false, const float* tp_d = nullptr);
 int limiter_validate(const mgb_limiter_params& lp);
 bool limiter_span_too_wide(const mgb_limiter_params& lp);  // the wide-window path serves these parameters
 int64_t limiter_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // its workspace planes; 0 for the halo kernel
@@ -164,10 +166,16 @@ int64_t limiter_wide_lookback_bytes(const mgb_limiter_params& lp, int64_t frames
 int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames);
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
-                        void* planes, const void* tables, cudaStream_t stream, bool gains_only);
+                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d);
 int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream_t stream);
 int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, double threshold, int* engaged,
                            cudaStream_t stream);
+
+// true_peak.cuh -----------------------------------------------------------------------------------
+void true_peak_filter(int oversample, double* h);  // the 12 L + 1 interpolator taps
+int64_t true_peak_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // the detector plane; 0 without true_peak
+int launch_true_peak_detect(int oversample, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream);
+int launch_true_peak_final(const float* d_max, double eps, double threshold, mgb_track_state* state, cudaStream_t stream);
 
 // fft test entry (api.cu) uses these -------------------------------------------------------------
 int launch_test_fft(int n, int is_f64, int dir, const void* in, void* out, int batch, const void* tw,

@@ -131,13 +131,15 @@ __global__ void limiter_tables_kernel(mgb_limiter_params lp, int span_ept, unsig
 // memory) or MGB_MAX_FILTER_ORDER = 2 (orders 1..2 zero-padded to 2; tables read through L1).
 // GAINS (tests only, mgb_test_limiter_gains): instead of the limited samples, write the two float64-scan results
 // per frame: (g_att, the attack filter's gain; max(hold_out, release_out), the release gain).
-template <int EPT, int NO, bool GAINS = false>
+// TP (true-peak mode, true_peak.cuh): P1 rectifies the detector plane tp_d instead of max(|L|, |R|); the samples are
+// read only where the output is formed.
+template <int EPT, int NO, bool GAINS = false, bool TP = false>
 // (two CTAs per SM where the span leaves room for them: up to 17 samples per thread at order capacity 1)
 __global__ void __launch_bounds__(NT, (NO == 1 && EPT <= 17) ? 2 : 1)
 limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__ in, float2* __restrict__ out,
                long long frames, const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
                const int* __restrict__ engaged, int* __restrict__ ticket, LookbackWord* __restrict__ slots,
-               const unsigned char* __restrict__ tables) {
+               const unsigned char* __restrict__ tables, const float* __restrict__ tp_d) {
     constexpr int HC = CORE_EPT + NO;  // H samples a thread needs: its core and the NO before it
     constexpr int CAP = EPT * NT;
     MGB_DYN_SMEM(smem);
@@ -183,7 +185,15 @@ limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__
     // All of the thread's loads go out first (one DRAM latency, not EPT), then the scalars and the tables: the
     // kernel's first use of anything it loaded comes after everything has been requested.
     float2 v[EPT];
-    {
+    float dv[TP ? EPT : 1];
+    if constexpr (TP) {
+        const float* base = tp_d + ga;
+#pragma unroll
+        for (int k = 0; k < EPT; ++k) {
+            const int i = tid + k * NT;
+            dv[k] = (i >= vlo && i < vhi) ? __ldg(base + i) : 0.0f;
+        }
+    } else {
         const float2* base = in + ga;
 #pragma unroll
         for (int k = 0; k < EPT; ++k) {
@@ -220,7 +230,9 @@ limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__
     for (int k = 0; k < EPT; ++k) {
         // g = 1 - thr/a = (a - thr)/a: the difference in float64 (it decides which frames are touched at
         // all, and cancels when a is close to thr), the quotient in float32 -- g is kept as float32 anyway
-        const double a = (double)fmaxf(fabsf(v[k].x), fabsf(v[k].y)) * pre;
+        double a;
+        if constexpr (TP) a = (double)dv[k] * pre;
+        else a = (double)fmaxf(fabsf(v[k].x), fabsf(v[k].y)) * pre;
         const double over = a - thr;
         float g = 0.0f;
         if (over > 0.0) g = __fdiv_rn((float)over, (float)a);
@@ -577,6 +589,8 @@ int limiter_validate(const mgb_limiter_params& lp) {
                 lp.release_order, MGB_MAX_FILTER_ORDER);
     MGB_REQUIRE(lp.attack_c > 0.0 && lp.attack_c < 1.0, MGB_ERR_INVALID, "limiter: attack pole out of (0,1)");
     MGB_REQUIRE(lp.threshold > 0.0, MGB_ERR_INVALID, "limiter: threshold must be positive");
+    MGB_REQUIRE(lp.true_peak == 0 || lp.true_peak == 1 || lp.true_peak == 2 || lp.true_peak == 4, MGB_ERR_INVALID,
+                "limiter: true_peak %d (0: sample peaks; 1, 2 or 4: the detector's oversampling)", lp.true_peak);
     return MGB_OK;
 }
 
@@ -745,13 +759,15 @@ int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream
 
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
                    const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
-                   const void* tables, cudaStream_t stream, bool gains_only) {
+                   const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d) {
     MGB_TRY(limiter_validate(lp));
     MGB_REQUIRE(frames > 6, MGB_ERR_INVALID, "limiter: the input must be longer than filtfilt's padlen (6)");
     MGB_REQUIRE(tables != nullptr, MGB_ERR_INVALID, "limiter: pole tables missing");
+    const bool tp = lp.true_peak != 0;
+    MGB_REQUIRE(!tp || tp_d != nullptr, MGB_ERR_INVALID, "limiter: true-peak mode without the detector plane");
     if (limiter_span_too_wide(lp))  // (chunks by block index: the wide-window path has no ticket)
         return launch_limiter_wide(lp, limiter_order_capacity(lp), g_lookback_inclusive, in, out, frames, pre_gain, post_gain,
-                                   engaged, lookback, wide_planes, tables, stream, gains_only);
+                                   engaged, lookback, wide_planes, tables, stream, gains_only, tp ? tp_d : nullptr);
     LimiterGeom g;
     MGB_TRY(limiter_geometry(lp, &g));
     const int64_t chunks = (frames + LC - 1) / LC;
@@ -761,23 +777,25 @@ int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, 
         auto go = [&](auto kernel) {
             return launch("limiter_kernel", kernel, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, in, out,
                           (long long)frames, pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback,
-                          (const unsigned char*)tables);
+                          (const unsigned char*)tables, tp_d);
         };
-        if (no == 1 && g.ept == 11) return go(limiter_kernel<11, 1, true>);
-        if (no == 1 && g.ept == 13) return go(limiter_kernel<13, 1, true>);
-        if (no == MGB_MAX_FILTER_ORDER && g.ept == 11) return go(limiter_kernel<11, MGB_MAX_FILTER_ORDER, true>);
+        if (no == 1 && g.ept == 11) return tp ? go(limiter_kernel<11, 1, true, true>) : go(limiter_kernel<11, 1, true>);
+        if (no == 1 && g.ept == 13) return tp ? go(limiter_kernel<13, 1, true, true>) : go(limiter_kernel<13, 1, true>);
+        if (no == MGB_MAX_FILTER_ORDER && g.ept == 11)
+            return tp ? go(limiter_kernel<11, MGB_MAX_FILTER_ORDER, true, true>) : go(limiter_kernel<11, MGB_MAX_FILTER_ORDER, true>);
         set_error("limiter gains (test entry): no kernel for %d span samples per thread at order capacity %d", g.ept, no);
         return MGB_ERR_UNSUPPORTED;
     }
+    auto run = [&](auto kernel) {
+        return launch("limiter_kernel", kernel, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, in, out, (long long)frames,
+                      pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback, (const unsigned char*)tables, tp_d);
+    };
 #define MGB_LIMITER_CASE(E)                                                                                           \
     case E:                                                                                                           \
-        if (no == 1)                                                                                                  \
-            return launch("limiter_kernel", limiter_kernel<E, 1>, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, in, \
-                          out, (long long)frames, pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback,     \
-                          (const unsigned char*)tables);                                                             \
-        return launch("limiter_kernel", limiter_kernel<E, MGB_MAX_FILTER_ORDER>, dim3((unsigned)chunks), dim3(NT), smem, \
-                      stream, lp, g, in, out, (long long)frames, pre_gain, post_gain, engaged, ticket,               \
-                      (LookbackWord*)lookback, (const unsigned char*)tables);
+        if (tp)                                                                                                       \
+            return no == 1 ? run(limiter_kernel<E, 1, false, true>)                                                   \
+                           : run(limiter_kernel<E, MGB_MAX_FILTER_ORDER, false, true>);                               \
+        return no == 1 ? run(limiter_kernel<E, 1>) : run(limiter_kernel<E, MGB_MAX_FILTER_ORDER>);
     switch (g.ept) {
         MGB_LIMITER_CASE(11)
         MGB_LIMITER_CASE(13)
@@ -803,3 +821,4 @@ int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, doubl
 }  // namespace mgb
 
 #include "loudness.cuh"  // the loudness meter: the same scans, look-back words and section tables
+#include "true_peak.cuh"  // the true-peak detector of the limiter's true-peak mode

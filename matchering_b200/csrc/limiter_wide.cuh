@@ -72,9 +72,11 @@ __device__ __forceinline__ float env_h(const WidePlanes& p, const WideGeom& w, l
 
 __device__ __forceinline__ bool bypassed(const int* engaged) { return engaged && *engaged == 0; }
 
+// TP: the true-peak mode's detector plane tp_d in place of max(|L|, |R|) (true_peak.cuh)
+template <bool TP>
 __global__ void __launch_bounds__(256) limiter_wide_gain_kernel(mgb_limiter_params lp, WideGeom w, const float2* __restrict__ in,
                                                                 const double* __restrict__ pre_gain, const int* __restrict__ engaged,
-                                                                WidePlanes p) {
+                                                                WidePlanes p, const float* __restrict__ tp_d) {
     if (bypassed(engaged)) return;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if ((i >> 5) >= w.nblocks) return;  // (whole warps)
@@ -83,8 +85,13 @@ __global__ void __launch_bounds__(256) limiter_wide_gain_kernel(mgb_limiter_para
     float g = 0.0f;
     if (i < w.frames) {
         // exactly the halo kernel's g (limiter.cu, P1)
-        const float2 v = __ldg(in + i);
-        const double a = (double)fmaxf(fabsf(v.x), fabsf(v.y)) * pre;
+        double a;
+        if constexpr (TP) {
+            a = (double)__ldg(tp_d + i) * pre;
+        } else {
+            const float2 v = __ldg(in + i);
+            a = (double)fmaxf(fabsf(v.x), fabsf(v.y)) * pre;
+        }
         const double over = a - lp.threshold;
         if (over > 0.0) g = __fdiv_rn((float)over, (float)a);
     }
@@ -417,7 +424,7 @@ int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames) {
 
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
-                        void* planes, const void* tables, cudaStream_t stream, bool gains_only) {
+                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d) {
     MGB_REQUIRE(planes != nullptr, MGB_ERR_INVALID, "limiter (wide windows): workspace planes missing");
     const WideLayout L = wide_layout(lp, frames);
     unsigned char* base = (unsigned char*)planes;
@@ -438,8 +445,13 @@ int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int pu
     const unsigned char* tab = (const unsigned char*)tables;
     LookbackWord* sec_words = (LookbackWord*)lookback;
     LookbackWord* att_words = sec_words + L.chunks * 2 * order_capacity;
-    MGB_TRY(launch("limiter_wide_gain_kernel", limiter_wide_gain_kernel, dim3((unsigned)((L.nblocks * 32 + 255) / 256)), dim3(256), 0,
-                   stream, lp, w, in, pre_gain, engaged, p));
+    const dim3 gain_grid((unsigned)((L.nblocks * 32 + 255) / 256));
+    if (tp_d)
+        MGB_TRY(launch("limiter_wide_gain_kernel", limiter_wide_gain_kernel<true>, gain_grid, dim3(256), 0, stream, lp, w, in, pre_gain,
+                       engaged, p, tp_d));
+    else
+        MGB_TRY(launch("limiter_wide_gain_kernel", limiter_wide_gain_kernel<false>, gain_grid, dim3(256), 0, stream, lp, w, in, pre_gain,
+                       engaged, p, tp_d));
     for (int level = 1; level <= L.levels; ++level)
         MGB_TRY(launch("limiter_wide_sparse_kernel", limiter_wide_sparse_kernel, dim3((unsigned)((L.nblocks + 255) / 256)), dim3(256), 0,
                        stream, w, engaged, p.st, level));

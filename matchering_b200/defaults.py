@@ -42,7 +42,7 @@ class Config:
                  lowess_frac: float = 0.0375, lowess_it: int = 0, lowess_delta: float = 0.001,
                  preview_size: float = 30, preview_analysis_step: float = 5, preview_fade_size: float = 1,
                  preview_fade_coefficient: float = 8, temp_folder: str = None,
-                 limiter: LimiterConfig = None):
+                 limiter: LimiterConfig = None, true_peak: bool = False):
         sr = internal_sample_rate
         _require(isinstance(sr, int) and sr > 0, "internal_sample_rate must be a positive int")
         if sr != 44100:
@@ -73,6 +73,7 @@ class Config:
         if limiter is None:
             limiter = _DEFAULT_LIMITER
         _require(isinstance(limiter, LimiterConfig), "limiter must be a LimiterConfig")
+        _require(isinstance(true_peak, bool), "true_peak must be a bool")
 
         self.internal_sample_rate = sr
         self.max_length = max_length
@@ -94,6 +95,9 @@ class Config:
         self.preview_fade_coefficient = preview_fade_coefficient
         self.temp_folder = temp_folder
         self.limiter = limiter
+        # True: the limiter, its early-out and the normalised output hold `threshold` on the true peak (the signal
+        # between samples, through the loudness meter's interpolator) instead of the sample peak
+        self.true_peak = true_peak
 
 
 _DEFAULT_LIMITER = LimiterConfig()  # shared default instance, like the reference's default argument

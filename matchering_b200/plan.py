@@ -209,6 +209,7 @@ class LimiterConstants:
     hold_a: np.ndarray
     release_b: np.ndarray
     release_a: np.ndarray
+    true_peak: int = 0  # mgb_limiter_params.true_peak: 0 (sample peaks) or the detector's oversampling factor L
 
 
 MAX_FILTER_ORDER = 2   # MGB_MAX_FILTER_ORDER
@@ -237,7 +238,9 @@ def limiter_constants(config) -> LimiterConstants:
     warmup = max(32, (warmup + 31) // 32 * 32)  # (the halo kernel's warm-up; wider windows take the wide-window path)
     bh, ah = _signal.butter(lim.hold_filter_order, lim.hold_filter_coefficient, fs=sr)
     br, ar = _signal.butter(lim.release_filter_order, lim.release_filter_coefficient / lim.release, fs=sr)
-    return LimiterConstants(config.threshold, reach, hold, warmup, c, bh, ah, br, ar)
+    # Config(true_peak=True): the meter's oversampling at this rate (loudness_constants)
+    tp = (4 if sr < 96000 else (2 if sr < 192000 else 1)) if getattr(config, "true_peak", False) else 0
+    return LimiterConstants(config.threshold, reach, hold, warmup, c, bh, ah, br, ar, tp)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -310,7 +313,7 @@ def config_key(config) -> tuple:
             config.rms_correction_steps, float(config.max_piece_size), config.threshold, config.min_value,
             config.lowess_frac, config.lowess_it, config.lowess_delta, lim.attack, lim.hold, lim.release,
             lim.attack_filter_coefficient, lim.hold_filter_order, lim.hold_filter_coefficient,
-            lim.release_filter_order, lim.release_filter_coefficient)
+            lim.release_filter_order, lim.release_filter_coefficient, bool(getattr(config, "true_peak", False)))
 
 
 def build_tables(config) -> PlanTables:
