@@ -506,6 +506,12 @@ int mgb_test_fft(int32_t n, int32_t is_f64, int32_t dir, const void* d_in, void*
  * takes the wide-window path (windows wider than the halo kernel's span). */
 int mgb_test_limiter_gains(const mgb_limiter_params* params, const float* d_in_lr, float* d_gains_out, int64_t frames,
                            void* d_workspace, int64_t workspace_bytes, int32_t* d_engaged, void* stream);
+/* the true-peak limiter's detector plane alone (the kernel mgb_limit runs in true-peak mode): d_out[n] = d[n] =
+ * max(u[n], u[n-1]) for the `frames` stereo frames at d_lr, oversampling 1, 2 or 4 (mgb_limiter_params.true_peak), and
+ * *d_max = max(*d_max, max(d)).  *d_max must hold 0 (or a smaller value) before the call.  Every pointer 16-byte
+ * aligned. */
+int mgb_test_true_peak_detect(int32_t oversample, const float* d_lr, int64_t frames, float* d_out, float* d_max,
+                              void* stream);
 /* the FIR design alone from given average spectra: d_avg = [4][n_lin] doubles
  * (target mid, target side, reference mid, reference side), already scaled. d_fir_out [2][F]. */
 int mgb_test_design_fir(const mgb_plan* plan, const double* d_avg, double* d_fir_out, void* d_workspace,

@@ -252,6 +252,7 @@ PROTOTYPES = {
                                C.c_int32, C.c_void_p]),
     "mgb_test_limiter_gains": (C.c_int, [C.POINTER(LimiterParams), C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                          C.c_void_p, C.c_void_p]),
+    "mgb_test_true_peak_detect": (C.c_int, [C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_test_fft": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                C.c_void_p]),
     "mgb_test_design_fir": (C.c_int, [C.POINTER(Plan), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

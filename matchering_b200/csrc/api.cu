@@ -769,6 +769,17 @@ int mgb_test_limiter_gains(const mgb_limiter_params* params, const float* d_in_l
     return limit_impl(params, d_in_lr, d_gains_out, frames, d_workspace, workspace_bytes, d_engaged, stream, true);
 }
 
+int mgb_test_true_peak_detect(int32_t oversample, const float* d_lr, int64_t frames, float* d_out, float* d_max,
+                              void* stream) {
+    MGB_REQUIRE(oversample == 1 || oversample == 2 || oversample == 4, MGB_ERR_INVALID,
+                "true_peak_detect: oversampling %d (1, 2 or 4)", oversample);
+    MGB_TRY(check_aligned(d_lr, "d_lr"));
+    MGB_TRY(check_aligned(d_out, "d_out"));
+    MGB_TRY(check_aligned(d_max, "d_max"));
+    MGB_REQUIRE(frames > 0, MGB_ERR_INVALID, "true_peak_detect: no frames");
+    return launch_true_peak_detect(oversample, (const float2*)d_lr, frames, d_out, d_max, (cudaStream_t)stream);
+}
+
 int mgb_process_host(const mgb_plan* plan, const mgb_track_layout* L, const float* h_target_lr,
                      const float* h_reference_lr, float* h_out_limited, float* h_out_no_limiter,
                      float* h_out_normalized, float* d_target_lr, float* d_reference_lr, float* d_result_lr,
