@@ -346,6 +346,53 @@ int64_t mgb_loudness_workspace_bytes(const mgb_loudness_params* params, int64_t 
 int mgb_loudness(const mgb_loudness_params* params, const float* d_lr, int64_t frames, void* d_workspace,
                  int64_t workspace_bytes, mgb_loudness_result* d_result, void* stream);
 
+/* ---- loudness targets: drive the limiter until the limited output reads a given integrated loudness ----
+ * Let s be the signal the limiter would take (mgb_finalize: result * gain, the correction gain; mgb_limit: the input),
+ * T the target (LUFS) and X the largest drive (dB).  The output is y(x) = limit(s * 10^(x/20)) at the drive x the search
+ * ends on, the unchanged limiter
+ * in the plan's (params') peak mode, WITHOUT final_amplitude_coefficient: that coefficient only carries a quiet
+ * reference's level, which the target replaces, and keeping it would move the ceiling below the threshold.  x* comes
+ * from a search on the device (one thread, float64; I = the meter's integrated loudness, f = I - T):
+ *   I_s = I(s).  -inf (silence, or no complete 400 ms window): one pass at x = 0, status UNDEFINED.
+ *   x_1 = min(T - I_s, X).  Pass k: limit at x_k, meter, f_k.  Stop on |f_k| <= MGB_LOUDNESS_TARGET_TOLERANCE
+ *   (REACHED), f_k < 0 at x_k >= X (UNREACHABLE), a bracket narrower than 1e-3 dB (BRACKET), MAX_PASSES passes
+ *   (PASSES), or I(y(x_k)) = -inf (UNDEFINED).  Otherwise the secant through the last two points (slope 1 on the first
+ *   pass, and where the secant's slope is not positive), held to at least x_lo - f_lo while only points below the
+ *   target are known and to at most x_hi - f_hi while only points above are known (a limiter cannot raise loudness
+ *   faster than 1 LU per dB), replaced by the bracket's midpoint where it leaves the open bracket, capped at X.
+ * The output holds the last pass's samples, and the report the loudness measured on them.  Every pass is launched
+ * (the host cannot know how many a track needs without a synchronisation); the kernels of a pass the search did
+ * not need return at once.  Nothing here synchronises. */
+#define MGB_LOUDNESS_TARGET_MAX_PASSES 8
+#define MGB_LOUDNESS_TARGET_TOLERANCE 0.01 /* LU */
+#define MGB_LOUDNESS_TARGET_MAX_GAIN_DB 48.0
+enum { MGB_LOUDNESS_REACHED = 1, MGB_LOUDNESS_UNREACHABLE = 2, MGB_LOUDNESS_BRACKET = 3, MGB_LOUDNESS_PASSES = 4,
+       MGB_LOUDNESS_UNDEFINED = 5 };
+typedef struct mgb_loudness_target {
+    double target_lufs;  /* finite, below 0 and above the absolute gate (-70 LUFS) */
+    double max_gain_db;  /* X, in [0, MGB_LOUDNESS_TARGET_MAX_GAIN_DB] */
+} mgb_loudness_target;
+typedef struct mgb_loudness_target_report {
+    double gain_db;          /* x*: drive into the limiter, on top of the correction gain */
+    double integrated;       /* I(y(x*)), LUFS, measured on the samples written */
+    double input_integrated; /* I_s */
+    double trace_gain_db[MGB_LOUDNESS_TARGET_MAX_PASSES], trace_integrated[MGB_LOUDNESS_TARGET_MAX_PASSES]; /* passes used */
+    int32_t passes, status;  /* MGB_LOUDNESS_REACHED / _UNREACHABLE / _BRACKET / _PASSES / _UNDEFINED */
+} mgb_loudness_target_report;
+/* The search's own workspace (a header, then the meter's workspace); -1 for bad arguments.  Needs no initialisation. */
+int64_t mgb_loudness_target_workspace_bytes(const mgb_loudness_params* meter, int64_t frames);
+/* Stage 4's limited output at the target, after mgb_correct_levels, into d_out_limited (which also serves as the
+ * search's scratch until the first pass, so it must not be d_result_lr: MGB_ERR_INVALID).  d_workspace is the job's; it keeps its layout.  d_report: device. */
+int mgb_finalize_to_loudness(const mgb_plan* plan, const mgb_track_layout* layout, const mgb_loudness_params* meter,
+                             const mgb_loudness_target* target, const float* d_result_lr, float* d_out_limited,
+                             void* d_workspace, void* d_search_ws, int64_t search_ws_bytes, mgb_track_state* d_state,
+                             mgb_loudness_target_report* d_report, void* stream);
+/* mgb_limit at the target; one workspace of mgb_limiter_workspace_bytes + mgb_loudness_target_workspace_bytes.  Every
+ * pass reads d_in_lr, so d_out_lr must be another buffer (MGB_ERR_INVALID). */
+int mgb_limit_to_loudness(const mgb_limiter_params* params, const mgb_loudness_params* meter, const mgb_loudness_target* target,
+                          const float* d_in_lr, float* d_out_lr, int64_t frames, void* d_workspace, int64_t workspace_bytes,
+                          mgb_loudness_target_report* d_report, void* stream);
+
 /* ---- whole job with HOST buffers (the call the end-to-end benchmark times) --------------------
  * h_* are host pointers (pinned for full speed).  Copies target and reference to the device,
  * runs stages 1-4 and copies the requested outputs back; synchronises `stream` before returning.
@@ -451,6 +498,15 @@ int mgb_pipeline_enable_loudness(mgb_pipeline* p, const mgb_loudness_params* par
 /* mgb_pipeline_wait, and the slot's meter (MGB_ERR_INVALID when metering is not enabled) */
 int mgb_pipeline_wait_loudness(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out,
                                mgb_loudness_result* loudness_out);
+/* Master every later submission's limited output at a loudness target (mgb_finalize_to_loudness in place of
+ * mgb_finalize, on the slot's compute stream); the slot's meter then meters the searched output and the report is copied
+ * back with the state and the meter.  Called after mgb_pipeline_enable_loudness (the search uses its meter) and before
+ * the first submit; MGB_ERR_INVALID otherwise, or for a target mgb_finalize_to_loudness would reject.  Allocates each
+ * slot's search workspace and report.  A pipeline that never calls this runs exactly what it did before. */
+int mgb_pipeline_enable_loudness_target(mgb_pipeline* p, const mgb_loudness_target* target);
+/* mgb_pipeline_wait_loudness, and the slot's loudness-target report (MGB_ERR_INVALID when no target is set) */
+int mgb_pipeline_wait_loudness_target(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out,
+                                      mgb_loudness_result* loudness_out, mgb_loudness_target_report* report_out);
 int mgb_pipeline_streams(mgb_pipeline* p, void** h2d, void** compute, void** d2h);
 int mgb_pipeline_destroy(mgb_pipeline* p);
 

@@ -168,6 +168,24 @@ class LoudnessResult(C.Structure):
     ]
 
 
+MGB_LOUDNESS_TARGET_MAX_PASSES = 8
+MGB_LOUDNESS_TARGET_TOLERANCE = 0.01
+MGB_LOUDNESS_REACHED, MGB_LOUDNESS_UNREACHABLE, MGB_LOUDNESS_BRACKET, MGB_LOUDNESS_PASSES, MGB_LOUDNESS_UNDEFINED = 1, 2, 3, 4, 5
+
+
+class LoudnessTargetParams(C.Structure):
+    _fields_ = [("target_lufs", C.c_double), ("max_gain_db", C.c_double)]
+
+
+class LoudnessTargetReport(C.Structure):
+    _fields_ = [
+        ("gain_db", C.c_double), ("integrated", C.c_double), ("input_integrated", C.c_double),
+        ("trace_gain_db", C.c_double * MGB_LOUDNESS_TARGET_MAX_PASSES),
+        ("trace_integrated", C.c_double * MGB_LOUDNESS_TARGET_MAX_PASSES),
+        ("passes", C.c_int32), ("status", C.c_int32),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/matchering_b200.h declares
 PROTOTYPES = {
     "mgb_version": (C.c_int, []),
@@ -237,6 +255,15 @@ PROTOTYPES = {
     "mgb_loudness_workspace_bytes": (C.c_int64, [C.POINTER(LoudnessParams), C.c_int64]),
     "mgb_loudness": (C.c_int, [C.POINTER(LoudnessParams), C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                C.c_void_p]),
+    "mgb_loudness_target_workspace_bytes": (C.c_int64, [C.POINTER(LoudnessParams), C.c_int64]),
+    "mgb_finalize_to_loudness": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.POINTER(LoudnessParams),
+                                           C.POINTER(LoudnessTargetParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mgb_limit_to_loudness": (C.c_int, [C.POINTER(LimiterParams), C.POINTER(LoudnessParams), C.POINTER(LoudnessTargetParams),
+                                        C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "mgb_pipeline_enable_loudness_target": (C.c_int, [C.c_void_p, C.POINTER(LoudnessTargetParams)]),
+    "mgb_pipeline_wait_loudness_target": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TrackState), C.POINTER(LoudnessResult),
+                                                    C.POINTER(LoudnessTargetReport)]),
     "mgb_pipeline_streams": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
     "mgb_pipeline_destroy": (C.c_int, [C.c_void_p]),
     "mgb_convert_f64_to_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),

@@ -15,7 +15,7 @@ import torch
 
 from . import _native
 from .engine import get_plan
-from .loudness import Loudness, device_meter
+from .loudness import Loudness, LoudnessTarget, debug_target, device_meter, target_params
 from .profile import ReferenceProfile
 
 
@@ -25,7 +25,9 @@ class MasteringPipeline:
         """max_reference_frames bounds the references submitted as samples; profiles have no such bound
         (a pipeline that only takes profiles may pass smallest_reference_frames(config)).
         loudness=True meters every limited output on the device (mg.loudness's meter, at the Config's rate)
-        and `wait_loudness` returns it."""
+        and `wait_loudness` returns it.  With Config(loudness_target=T) every limited output is driven to T LUFS
+        (mgb_pipeline_enable_loudness_target; its search uses the meter, which is then always on) and
+        `wait_loudness_target` returns the meter and the search's report."""
         self.config = config
         self.plan = get_plan(config, device)
         self.lib = self.plan.lib
@@ -33,13 +35,17 @@ class MasteringPipeline:
         self.depth = depth
         self._handle = C.c_void_p()
         # (the meter's tables are cached per device and rate: they outlive the pipeline)
-        self._meter = device_meter(config.internal_sample_rate, self.device) if loudness else None
+        self.target = getattr(config, "loudness_target", None)
+        self._meter = (device_meter(config.internal_sample_rate, self.device)
+                       if loudness or self.target is not None else None)
         self._pending = {}  # slot -> (target, reference, out) kept alive until the slot is waited on
         with torch.cuda.device(self.device):
             _native.check(self.lib, self.lib.mgb_pipeline_create(C.byref(self.plan.struct), max_target_frames,
                                                                  max_reference_frames, depth, C.byref(self._handle)))
-            if loudness:
+            if self._meter is not None:
                 status = self.lib.mgb_pipeline_enable_loudness(self._handle, C.byref(self._meter.params))
+                if status == _native.MGB_OK and self.target is not None:
+                    status = self.lib.mgb_pipeline_enable_loudness_target(self._handle, C.byref(target_params(self.target)))
                 if status != _native.MGB_OK:
                     self.close()
                     _native.check(self.lib, status)
@@ -124,6 +130,17 @@ class MasteringPipeline:
         self._pending.pop(slot, None)
         return st, Loudness.from_result(res)
 
+    def wait_loudness_target(self, slot: int) -> tuple:
+        """wait(slot), the meter of the slot's limited output and how its loudness search ended:
+        (TrackState, Loudness, LoudnessTarget).  Needs a Config with loudness_target."""
+        if self.target is None:
+            raise ValueError("this pipeline's Config has no loudness_target")
+        st, res, rep = _native.TrackState(), _native.LoudnessResult(), _native.LoudnessTargetReport()
+        _native.check(self.lib, self.lib.mgb_pipeline_wait_loudness_target(self._handle, slot, C.byref(st), C.byref(res),
+                                                                            C.byref(rep)))
+        self._pending.pop(slot, None)
+        return st, Loudness.from_result(res), LoudnessTarget.from_report(self.target, rep)
+
     def wait_all(self) -> None:
         for slot in list(self._pending):
             self.wait(slot)
@@ -154,7 +171,8 @@ def smallest_reference_frames(config) -> int:
 def master_many(pairs, config, depth: int = 3, loudness: bool = False):
     """[(target, reference), ...] float32 host arrays -> list of limited results (numpy float32).  A reference
     may be a ReferenceProfile (an album against one reference: analysed once, never copied again).
-    loudness=True returns (results, meters): each result's Loudness, metered on the device."""
+    loudness=True returns (results, meters): each result's Loudness, metered on the device.  With
+    Config(loudness_target=T) every result is driven to T LUFS; how each search ended goes to the debug log."""
     pairs = list(pairs)
     if not pairs:
         return ([], []) if loudness else []
@@ -165,17 +183,25 @@ def master_many(pairs, config, depth: int = 3, loudness: bool = False):
     max_r = max((len(r) for _, r in pairs if not isinstance(r, ReferenceProfile)), default=smallest_reference_frames(config))
     outs = [np.empty((len(t), 2), dtype=np.float32) for t, _ in pairs]
     meters = [None] * len(pairs)
+    target = getattr(config, "loudness_target", None) is not None
+
+    def collect(pipe, slot, k):
+        if target:
+            _, meters[k], t = pipe.wait_loudness_target(slot)
+            debug_target(t)
+        else:
+            meters[k] = pipe.wait_loudness(slot)[1]
+
     with MasteringPipeline(config, max_t, max_r, depth, loudness=loudness) as pipe:
         in_flight = []  # (slot, track) in submission order; slots are reused round-robin
         for i, ((t, r), o) in enumerate(zip(pairs, outs)):
             if not isinstance(r, ReferenceProfile):
                 r = np.ascontiguousarray(r, dtype=np.float32)
-            if loudness and len(in_flight) == depth:  # collect the meter of the slot this submit reuses
-                slot, k = in_flight.pop(0)
-                meters[k] = pipe.wait_loudness(slot)[1]
+            if (loudness or target) and len(in_flight) == depth:  # collect the slot this submit reuses
+                collect(pipe, *in_flight.pop(0))
             in_flight.append((pipe.submit(np.ascontiguousarray(t, dtype=np.float32), r, o), i))
-        if loudness:
+        if loudness or target:
             for slot, k in in_flight:
-                meters[k] = pipe.wait_loudness(slot)[1]
+                collect(pipe, slot, k)
         pipe.wait_all()
     return (outs, meters) if loudness else outs

@@ -708,6 +708,48 @@ int mgb_finalize(const mgb_plan* plan, const mgb_track_layout* L, const float* d
     return MGB_OK;
 }
 
+int mgb_finalize_to_loudness(const mgb_plan* plan, const mgb_track_layout* L, const mgb_loudness_params* meter,
+                             const mgb_loudness_target* target, const float* d_result_lr, float* d_out_limited,
+                             void* d_workspace, void* d_search_ws, int64_t search_ws_bytes, mgb_track_state* d_state,
+                             mgb_loudness_target_report* d_report, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_TRY(loudness_target_validate(target, meter));
+    MGB_REQUIRE(meter->sample_rate == plan->sample_rate, MGB_ERR_INVALID,
+                "finalize_to_loudness: the meter's rate %d differs from the plan's %d", meter->sample_rate, plan->sample_rate);
+    MGB_REQUIRE(plan->d_limiter_tables != nullptr, MGB_ERR_INVALID, "finalize_to_loudness: the plan has no limiter tables");
+    MGB_TRY(check_aligned(d_result_lr, "d_result_lr"));
+    MGB_TRY(check_aligned(d_out_limited, "d_out_limited"));
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_search_ws, "d_search_ws"));
+    MGB_TRY(check_aligned(d_report, "d_report"));
+    // (s = result * gain is staged in d_out_limited while every pass still reads the result)
+    MGB_REQUIRE((const void*)d_out_limited != (const void*)d_result_lr, MGB_ERR_INVALID,
+                "finalize_to_loudness: d_out_limited must not be d_result_lr (the output is the search's scratch)");
+    const int64_t need = loudness_target_search_bytes(*meter, L->target_frames);
+    MGB_REQUIRE(search_ws_bytes >= need, MGB_ERR_WORKSPACE, "finalize_to_loudness: search workspace of %lld bytes, need %lld",
+                (long long)search_ws_bytes, (long long)need);
+    cudaStream_t st = (cudaStream_t)stream;
+    Workspace ws = carve_workspace(*plan, *L, d_workspace);
+    const float2* res = (const float2*)d_result_lr;
+    const int64_t n = L->target_frames;
+    const bool tp = plan->limiter.true_peak != 0;
+    if (tp) {  // the detector once, over the result: d is linear in the input and the limiter scales it by its pre-gain
+#ifdef MGB_EMULATE
+        memset(ws.tickets, 0, ws.limiter_zero_bytes);
+#else
+        if (cudaMemsetAsync(ws.tickets, 0, ws.limiter_zero_bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+        MGB_TRY(launch_true_peak_detect(plan->limiter.true_peak, res, n, ws.tp_plane, ws.tp_peak, st));
+    }
+    // s = result * gain, metered once from d_out_limited (the first pass overwrites it)
+    MGB_TRY(launch_scale(res, (float2*)d_out_limited, n, &d_state->gain, nullptr, st));
+    return run_loudness_search(plan->limiter, *meter, *target, res, (const float2*)d_out_limited, (float2*)d_out_limited, n,
+                               &d_state->gain, tp ? nullptr : &d_state->result_peak, tp ? ws.tp_peak : nullptr, ws.tickets,
+                               ws.limiter_zero_bytes, nullptr, ws.lookback, ws.limiter_planes, plan->d_limiter_tables,
+                               tp ? ws.tp_plane : nullptr, d_search_ws, d_report, st);
+}
+
 // standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [32,36): the true-peak detector's maximum  [256, kLimitHeader):
 // pole tables  [kLimitHeader, ...): look-back words, then the wide-window path's planes (none for the halo kernel), then the
 // true-peak detector's plane (true-peak mode only)

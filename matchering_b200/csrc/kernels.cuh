@@ -156,7 +156,8 @@ int launch_convert_f32_f64(const float* in, double* out, int64_t count, cudaStre
 // (the halo kernel where its span fits, the wide-window path otherwise; wide_planes: limiter_plane_bytes of workspace)
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
                    const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
-                   const void* tables, cudaStream_t stream, bool gains_only = false, const float* tp_d = nullptr);
+                   const void* tables, cudaStream_t stream, bool gains_only = false, const float* tp_d = nullptr,
+                   const int* skip = nullptr);  // skip: gated kernels that return at once while *skip != 0
 int limiter_validate(const mgb_limiter_params& lp);
 bool limiter_span_too_wide(const mgb_limiter_params& lp);  // the wide-window path serves these parameters
 int64_t limiter_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // its workspace planes; 0 for the halo kernel
@@ -166,7 +167,8 @@ int64_t limiter_wide_lookback_bytes(const mgb_limiter_params& lp, int64_t frames
 int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames);
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
-                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d);
+                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d,
+                        const int* skip);
 int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream_t stream);
 int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, double threshold, int* engaged,
                            cudaStream_t stream);
@@ -176,6 +178,15 @@ void true_peak_filter(int oversample, double* h);  // the 12 L + 1 interpolator 
 int64_t true_peak_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // the detector plane; 0 without true_peak
 int launch_true_peak_detect(int oversample, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream);
 int launch_true_peak_final(const float* d_max, double eps, double threshold, mgb_track_state* state, cudaStream_t stream);
+
+// loudness_target.cuh -------------------------------------------------------------------------------
+int loudness_target_validate(const mgb_loudness_target* target, const mgb_loudness_params* meter);
+int64_t loudness_target_search_bytes(const mgb_loudness_params& meter, int64_t frames);
+int run_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& target,
+                        const float2* in, const float2* s_metered, float2* out, int64_t frames, const double* gain,
+                        const double* peak_d, const float* peak_bits, void* zero, int64_t zero_bytes, int* ticket,
+                        void* lookback, void* planes, const void* tables, const float* tp_d, void* search_ws,
+                        mgb_loudness_target_report* report, cudaStream_t stream);
 
 // fft test entry (api.cu) uses these -------------------------------------------------------------
 int launch_test_fft(int n, int is_f64, int dir, const void* in, void* out, int batch, const void* tw,

@@ -133,13 +133,18 @@ __global__ void limiter_tables_kernel(mgb_limiter_params lp, int span_ept, unsig
 // per frame: (g_att, the attack filter's gain; max(hold_out, release_out), the release gain).
 // TP (true-peak mode, true_peak.cuh): P1 rectifies the detector plane tp_d instead of max(|L|, |R|); the samples are
 // read only where the output is formed.
-template <int EPT, int NO, bool GAINS = false, bool TP = false>
+// GATED (loudness targets, loudness_target.cuh): the whole grid returns at once while *skip is set -- a pass the
+// search did not need.
+template <int EPT, int NO, bool GAINS = false, bool TP = false, bool GATED = false>
 // (two CTAs per SM where the span leaves room for them: up to 17 samples per thread at order capacity 1)
 __global__ void __launch_bounds__(NT, (NO == 1 && EPT <= 17) ? 2 : 1)
 limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__ in, float2* __restrict__ out,
                long long frames, const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
                const int* __restrict__ engaged, int* __restrict__ ticket, LookbackWord* __restrict__ slots,
-               const unsigned char* __restrict__ tables, const float* __restrict__ tp_d) {
+               const unsigned char* __restrict__ tables, const float* __restrict__ tp_d, const int* __restrict__ skip) {
+    if constexpr (GATED) {
+        if (*skip) return;
+    }
     constexpr int HC = CORE_EPT + NO;  // H samples a thread needs: its core and the NO before it
     constexpr int CAP = EPT * NT;
     MGB_DYN_SMEM(smem);
@@ -759,7 +764,7 @@ int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream
 
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
                    const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
-                   const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d) {
+                   const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d, const int* skip) {
     MGB_TRY(limiter_validate(lp));
     MGB_REQUIRE(frames > 6, MGB_ERR_INVALID, "limiter: the input must be longer than filtfilt's padlen (6)");
     MGB_REQUIRE(tables != nullptr, MGB_ERR_INVALID, "limiter: pole tables missing");
@@ -767,17 +772,18 @@ int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, 
     MGB_REQUIRE(!tp || tp_d != nullptr, MGB_ERR_INVALID, "limiter: true-peak mode without the detector plane");
     if (limiter_span_too_wide(lp))  // (chunks by block index: the wide-window path has no ticket)
         return launch_limiter_wide(lp, limiter_order_capacity(lp), g_lookback_inclusive, in, out, frames, pre_gain, post_gain,
-                                   engaged, lookback, wide_planes, tables, stream, gains_only, tp ? tp_d : nullptr);
+                                   engaged, lookback, wide_planes, tables, stream, gains_only, tp ? tp_d : nullptr, skip);
     LimiterGeom g;
     MGB_TRY(limiter_geometry(lp, &g));
     const int64_t chunks = (frames + LC - 1) / LC;
     const size_t smem = (size_t)g.ept * NT * 16 + (size_t)g.margin * 8;
     const int no = limiter_order_capacity(lp);
+    MGB_REQUIRE(!(gains_only && skip), MGB_ERR_INVALID, "limiter: the gains test entry has no gated passes");
     if (gains_only) {  // test entry: the sample rates of the golden vectors (44.1 and 96 kHz windows), both capacities
         auto go = [&](auto kernel) {
             return launch("limiter_kernel", kernel, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, in, out,
                           (long long)frames, pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback,
-                          (const unsigned char*)tables, tp_d);
+                          (const unsigned char*)tables, tp_d, skip);
         };
         if (no == 1 && g.ept == 11) return tp ? go(limiter_kernel<11, 1, true, true>) : go(limiter_kernel<11, 1, true>);
         if (no == 1 && g.ept == 13) return tp ? go(limiter_kernel<13, 1, true, true>) : go(limiter_kernel<13, 1, true>);
@@ -788,10 +794,18 @@ int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, 
     }
     auto run = [&](auto kernel) {
         return launch("limiter_kernel", kernel, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, in, out, (long long)frames,
-                      pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback, (const unsigned char*)tables, tp_d);
+                      pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback, (const unsigned char*)tables, tp_d, skip);
     };
+    // (gated passes of a loudness-target search: the same kernels behind the skip flag)
 #define MGB_LIMITER_CASE(E)                                                                                           \
     case E:                                                                                                           \
+        if (skip) {                                                                                                   \
+            if (tp)                                                                                                   \
+                return no == 1 ? run(limiter_kernel<E, 1, false, true, true>)                                         \
+                               : run(limiter_kernel<E, MGB_MAX_FILTER_ORDER, false, true, true>);                     \
+            return no == 1 ? run(limiter_kernel<E, 1, false, false, true>)                                            \
+                           : run(limiter_kernel<E, MGB_MAX_FILTER_ORDER, false, false, true>);                        \
+        }                                                                                                             \
         if (tp)                                                                                                       \
             return no == 1 ? run(limiter_kernel<E, 1, false, true>)                                                   \
                            : run(limiter_kernel<E, MGB_MAX_FILTER_ORDER, false, true>);                               \
@@ -822,3 +836,4 @@ int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, doubl
 
 #include "loudness.cuh"  // the loudness meter: the same scans, look-back words and section tables
 #include "true_peak.cuh"  // the true-peak detector of the limiter's true-peak mode
+#include "loudness_target.cuh"  // loudness targets: the search around the limiter and the meter

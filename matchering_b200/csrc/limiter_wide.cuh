@@ -72,11 +72,20 @@ __device__ __forceinline__ float env_h(const WidePlanes& p, const WideGeom& w, l
 
 __device__ __forceinline__ bool bypassed(const int* engaged) { return engaged && *engaged == 0; }
 
+// GATED (every kernel of this path, loudness_target.cuh): the grid returns at once while *skip is set
+template <bool GATED>
+__device__ __forceinline__ bool skipped(const int* skip) {
+    if constexpr (GATED) return *skip != 0;
+    return false;
+}
+
 // TP: the true-peak mode's detector plane tp_d in place of max(|L|, |R|) (true_peak.cuh)
-template <bool TP>
+template <bool TP, bool GATED = false>
 __global__ void __launch_bounds__(256) limiter_wide_gain_kernel(mgb_limiter_params lp, WideGeom w, const float2* __restrict__ in,
                                                                 const double* __restrict__ pre_gain, const int* __restrict__ engaged,
-                                                                WidePlanes p, const float* __restrict__ tp_d) {
+                                                                WidePlanes p, const float* __restrict__ tp_d,
+                                                                const int* __restrict__ skip) {
+    if (skipped<GATED>(skip)) return;
     if (bypassed(engaged)) return;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if ((i >> 5) >= w.nblocks) return;  // (whole warps)
@@ -111,7 +120,10 @@ __global__ void __launch_bounds__(256) limiter_wide_gain_kernel(mgb_limiter_para
     if (lane == 31) p.st[i >> 5] = pf;
 }
 
-__global__ void __launch_bounds__(256) limiter_wide_sparse_kernel(WideGeom w, const int* __restrict__ engaged, float* st, int level) {
+template <bool GATED = false>
+__global__ void __launch_bounds__(256) limiter_wide_sparse_kernel(WideGeom w, const int* __restrict__ engaged, float* st, int level,
+                                                                  const int* __restrict__ skip) {
+    if (skipped<GATED>(skip)) return;
     if (bypassed(engaged)) return;
     const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= w.nblocks) return;
@@ -126,13 +138,14 @@ __global__ void __launch_bounds__(256) limiter_wide_sparse_kernel(WideGeom w, co
 // forward plane.  BACKWARD = true: runs over the forward plane from its end (block b owns the b-th chunk counted from
 // the end), state beyond the last sample = its forward value; writes g_att for the signal's own samples.
 // words: [chunks][2] look-back words, forward pass in word 0 of its chunk, backward pass in word 1.
-template <bool BACKWARD>
+template <bool BACKWARD, bool GATED = false>
 __global__ void __launch_bounds__(NT) limiter_wide_attack_kernel(mgb_limiter_params lp, WideGeom w, const int* __restrict__ engaged,
                                                                  WidePlanes p, LookbackWord* __restrict__ words,
-                                                                 const unsigned char* __restrict__ tables) {
+                                                                 const unsigned char* __restrict__ tables, const int* __restrict__ skip) {
     __shared__ SectionTab<1> tab;  // the attack pole's powers in the sections' layout
     __shared__ double scratch[32];
     __shared__ double bcast;
+    if (skipped<GATED>(skip)) return;
     if (bypassed(engaged)) return;
     const int tid = threadIdx.x;
     {
@@ -210,12 +223,13 @@ __global__ void __launch_bounds__(NT) limiter_wide_attack_kernel(mgb_limiter_par
 
 // Hold and release sections (limiter.cu, P3 / P5 / P6: the same scans and look-back) over H from the window
 // maxima, then the gain and its application (P7).  GAINS (tests): write (g_att, max(hold_out, release_out)).
-template <int NO, bool GAINS>
+template <int NO, bool GAINS, bool GATED = false>
 __global__ void __launch_bounds__(NT) limiter_wide_apply_kernel(mgb_limiter_params lp, WideGeom w, const float2* __restrict__ in,
                                                                 float2* __restrict__ out, const double* __restrict__ pre_gain,
                                                                 const double* __restrict__ post_gain, const int* __restrict__ engaged,
                                                                 WidePlanes p, LookbackWord* __restrict__ slots,
-                                                                const unsigned char* __restrict__ tables) {
+                                                                const unsigned char* __restrict__ tables, const int* __restrict__ skip) {
+    if (skipped<GATED>(skip)) return;
     constexpr int HC = CORE_EPT + NO;
     __shared__ SectionTab<1> pw_sec[2];  // (order capacity 1 only: the two sections' tables)
     __shared__ double scratch_a[32 * NO], scratch_b[32 * NO];
@@ -424,7 +438,8 @@ int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames) {
 
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
-                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d) {
+                        void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d,
+                        const int* skip) {
     MGB_REQUIRE(planes != nullptr, MGB_ERR_INVALID, "limiter (wide windows): workspace planes missing");
     const WideLayout L = wide_layout(lp, frames);
     unsigned char* base = (unsigned char*)planes;
@@ -446,23 +461,32 @@ int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int pu
     LookbackWord* sec_words = (LookbackWord*)lookback;
     LookbackWord* att_words = sec_words + L.chunks * 2 * order_capacity;
     const dim3 gain_grid((unsigned)((L.nblocks * 32 + 255) / 256));
-    if (tp_d)
-        MGB_TRY(launch("limiter_wide_gain_kernel", limiter_wide_gain_kernel<true>, gain_grid, dim3(256), 0, stream, lp, w, in, pre_gain,
-                       engaged, p, tp_d));
-    else
-        MGB_TRY(launch("limiter_wide_gain_kernel", limiter_wide_gain_kernel<false>, gain_grid, dim3(256), 0, stream, lp, w, in, pre_gain,
-                       engaged, p, tp_d));
-    for (int level = 1; level <= L.levels; ++level)
-        MGB_TRY(launch("limiter_wide_sparse_kernel", limiter_wide_sparse_kernel, dim3((unsigned)((L.nblocks + 255) / 256)), dim3(256), 0,
-                       stream, w, engaged, p.st, level));
-    MGB_TRY(launch("limiter_wide_attack_kernel", limiter_wide_attack_kernel<false>, dim3((unsigned)L.ext_chunks), dim3(NT), 0, stream,
-                   lp, w, engaged, p, att_words, tab));
-    MGB_TRY(launch("limiter_wide_attack_kernel", limiter_wide_attack_kernel<true>, dim3((unsigned)L.ext_chunks), dim3(NT), 0, stream,
-                   lp, w, engaged, p, att_words, tab));
+    // (skip != null: the gated instances of a loudness-target search's passes; never with gains_only)
+    auto gain = [&](auto kernel) {
+        return launch("limiter_wide_gain_kernel", kernel, gain_grid, dim3(256), 0, stream, lp, w, in, pre_gain, engaged, p, tp_d, skip);
+    };
+    if (skip) MGB_TRY(tp_d ? gain(limiter_wide_gain_kernel<true, true>) : gain(limiter_wide_gain_kernel<false, true>));
+    else MGB_TRY(tp_d ? gain(limiter_wide_gain_kernel<true>) : gain(limiter_wide_gain_kernel<false>));
+    for (int level = 1; level <= L.levels; ++level) {
+        auto sparse = [&](auto kernel) {
+            return launch("limiter_wide_sparse_kernel", kernel, dim3((unsigned)((L.nblocks + 255) / 256)), dim3(256), 0, stream, w,
+                          engaged, p.st, level, skip);
+        };
+        MGB_TRY(skip ? sparse(limiter_wide_sparse_kernel<true>) : sparse(limiter_wide_sparse_kernel<>));
+    }
+    auto attack = [&](auto kernel) {
+        return launch("limiter_wide_attack_kernel", kernel, dim3((unsigned)L.ext_chunks), dim3(NT), 0, stream, lp, w, engaged, p,
+                      att_words, tab, skip);
+    };
+    MGB_TRY(skip ? attack(limiter_wide_attack_kernel<false, true>) : attack(limiter_wide_attack_kernel<false>));
+    MGB_TRY(skip ? attack(limiter_wide_attack_kernel<true, true>) : attack(limiter_wide_attack_kernel<true>));
     auto go = [&](auto kernel) {
         return launch("limiter_wide_apply_kernel", kernel, dim3((unsigned)L.chunks), dim3(NT), 0, stream, lp, w, in, out, pre_gain,
-                      post_gain, engaged, p, sec_words, tab);
+                      post_gain, engaged, p, sec_words, tab, skip);
     };
+    if (skip)
+        return order_capacity == 1 ? go(limiter_wide_apply_kernel<1, false, true>)
+                                   : go(limiter_wide_apply_kernel<MGB_MAX_FILTER_ORDER, false, true>);
     if (order_capacity == 1) return gains_only ? go(limiter_wide_apply_kernel<1, true>) : go(limiter_wide_apply_kernel<1, false>);
     return gains_only ? go(limiter_wide_apply_kernel<MGB_MAX_FILTER_ORDER, true>) : go(limiter_wide_apply_kernel<MGB_MAX_FILTER_ORDER, false>);
 }

@@ -197,16 +197,22 @@ __device__ __forceinline__ double tp_centre(const mgb_loudness_params& lp, const
     return m;
 }
 
-template <int OS>
+// GATED (every kernel of the meter, loudness_target.cuh): the grid returns at once while *skip is set -- a pass of a
+// loudness-target search that the search did not need
+template <int OS, bool GATED = false>
 __global__ void __launch_bounds__(NT) loudness_kernel(mgb_loudness_params lp, const float2* __restrict__ x, long long frames,
                                                       LookbackWord* __restrict__ words, double* __restrict__ part,
-                                                      double* __restrict__ peak, const MeterTables* __restrict__ tabs) {
+                                                      double* __restrict__ peak, const MeterTables* __restrict__ tabs,
+                                                      const int* __restrict__ skip) {
     __shared__ float2 xs[kMeterSpan];  // frames s0 - 6 .. s0 + LC + 5, zero outside the signal
     __shared__ double scratch[4][32 * 2];
     __shared__ double bcast[4];
     __shared__ double wsum[NT / 32][2];
     __shared__ int wsub[NT / 32];
     __shared__ double wmax[NT / 32][4];
+    if constexpr (GATED) {
+        if (*skip) return;
+    }
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int chunk = blockIdx.x;  // (the look-back waits on lower chunks only: blocks start in index order)
     const long long s0 = (long long)chunk * LC;
@@ -323,7 +329,12 @@ __global__ void __launch_bounds__(NT) loudness_kernel(mgb_loudness_params lp, co
 }
 
 // e_b = the shares of the chunks that touch sub-block b, in chunk order
-__global__ void loudness_fold_kernel(long long block, long long nb, const double* __restrict__ part, double* __restrict__ energy) {
+template <bool GATED = false>
+__global__ void loudness_fold_kernel(long long block, long long nb, const double* __restrict__ part, double* __restrict__ energy,
+                                     const int* __restrict__ skip) {
+    if constexpr (GATED) {
+        if (*skip) return;
+    }
     const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb) return;
     const long long lo = b * block, c0 = lo / LC, c1 = (lo + block - 1) / LC;
@@ -332,15 +343,20 @@ __global__ void loudness_fold_kernel(long long block, long long nb, const double
     energy[b] = e;
 }
 
+// (GATED: momentary windows only -- a search's pass meters integrated loudness alone)
+template <bool GATED = false>
 __global__ void loudness_windows_kernel(long long block, long long nb, const double* __restrict__ energy,
-                                        double* __restrict__ mom, double* __restrict__ st) {
+                                        double* __restrict__ mom, double* __restrict__ st, const int* __restrict__ skip) {
+    if constexpr (GATED) {
+        if (*skip) return;
+    }
     const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (j + 4 <= nb) {
         double s = 0.0;
         for (int i = 0; i < 4; ++i) s += energy[j + i];
         mom[j] = s / (4.0 * (double)block);
     }
-    if (j + 30 <= nb) {
+    if (!GATED && j + 30 <= nb) {
         double s = 0.0;
         for (int i = 0; i < 30; ++i) s += energy[j + i];
         st[j] = s / (30.0 * (double)block);
@@ -357,7 +373,8 @@ __global__ void __launch_bounds__(kMeterFinishThreads) loudness_finish_kernel(lo
     const int tid = threadIdx.x, nt = blockDim.x;
     const double neg_inf = -INFINITY;
 
-    // integrated loudness: absolute gate at -70 LUFS, relative gate 10 LU below the mean of what passed
+    // integrated loudness: absolute gate at -70 LUFS, relative gate 10 LU below the mean of what passed (repeated by
+    // loudness_integrated_kernel below: change both together; the loudness-target tests compare the two to the bit)
     double sa = 0.0, ca = 0.0, mmax = 0.0;
     for (long long j = tid; j < nm; j += nt) {
         const double z = mom[j];
@@ -440,6 +457,44 @@ __global__ void __launch_bounds__(kMeterFinishThreads) loudness_finish_kernel(lo
     }
 }
 
+// loudness_finish_kernel's integrated loudness alone, into *integrated_out (a loudness-target search's pass meter, gated
+// like the GATED kernels above).  Its own kernel rather than a flag on, or a helper shared with, the finish kernel: a
+// template flag there reordered two of the finish kernel's instructions, and the finish kernel stays unchanged to the
+// instruction.  The gate below is the finish kernel's, in the same order (change both together).
+__global__ void __launch_bounds__(kMeterFinishThreads) loudness_integrated_kernel(long long nm, const double* __restrict__ mom,
+                                                                                  const int* __restrict__ skip,
+                                                                                  double* __restrict__ integrated_out) {
+    __shared__ double red[32];
+    if (*skip) return;
+    const int tid = threadIdx.x, nt = blockDim.x;
+    double sa = 0.0, ca = 0.0;
+    for (long long j = tid; j < nm; j += nt) {
+        const double z = mom[j];
+        if (lufs(z) > -70.0) {
+            sa += z;
+            ca += 1.0;
+        }
+    }
+    sa = block_sum(sa, red);
+    ca = block_sum(ca, red);
+    double integrated = -INFINITY;
+    if (ca > 0.0) {
+        const double gate = lufs(sa / ca) - 10.0;
+        double sr = 0.0, cr = 0.0;
+        for (long long j = tid; j < nm; j += nt) {
+            const double z = mom[j], l = lufs(z);
+            if (l > -70.0 && l > gate) {
+                sr += z;
+                cr += 1.0;
+            }
+        }
+        sr = block_sum(sr, red);
+        cr = block_sum(cr, red);
+        if (cr > 0.0) integrated = lufs(sr / cr);
+    }
+    if (tid == 0) *integrated_out = integrated;
+}
+
 int loudness_validate(const mgb_loudness_params* lp) {
     MGB_REQUIRE(lp != nullptr, MGB_ERR_INVALID, "loudness: params is NULL");
     MGB_REQUIRE(lp->sample_rate >= 8000 && lp->sample_rate <= 384000, MGB_ERR_INVALID,
@@ -504,20 +559,21 @@ int mgb_loudness(const mgb_loudness_params* params, const float* d_lr, int64_t f
     const float2* x = (const float2*)d_lr;
     const MeterTables* tabs = (const MeterTables*)params->d_tables;
     const dim3 grid((unsigned)w.chunks);
+    const int* no_skip = nullptr;
     if (lp.oversample == 4)
         MGB_TRY(launch("loudness_kernel", loudness_kernel<4>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs));
+                       w.part, w.peak, tabs, no_skip));
     else if (lp.oversample == 2)
         MGB_TRY(launch("loudness_kernel", loudness_kernel<2>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs));
+                       w.part, w.peak, tabs, no_skip));
     else
         MGB_TRY(launch("loudness_kernel", loudness_kernel<1>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs));
+                       w.part, w.peak, tabs, no_skip));
     const long long B = lp.block;
-    MGB_TRY(launch("loudness_fold_kernel", loudness_fold_kernel, dim3((unsigned)((w.nb + 255) / 256)), dim3(256), 0, st, B,
-                   (long long)w.nb, (const double*)w.part, w.energy));
-    MGB_TRY(launch("loudness_windows_kernel", loudness_windows_kernel, dim3((unsigned)((w.nm + 255) / 256)), dim3(256), 0, st,
-                   B, (long long)w.nb, (const double*)w.energy, w.mom, w.st));
+    MGB_TRY(launch("loudness_fold_kernel", loudness_fold_kernel<>, dim3((unsigned)((w.nb + 255) / 256)), dim3(256), 0, st, B,
+                   (long long)w.nb, (const double*)w.part, w.energy, no_skip));
+    MGB_TRY(launch("loudness_windows_kernel", loudness_windows_kernel<>, dim3((unsigned)((w.nm + 255) / 256)), dim3(256), 0, st,
+                   B, (long long)w.nb, (const double*)w.energy, w.mom, w.st, no_skip));
     return launch("loudness_finish_kernel", loudness_finish_kernel, dim3(1), dim3(kMeterFinishThreads), 0, st,
                   (long long)w.chunks, (long long)w.nm, (long long)w.ns, (const double*)w.peak, (const double*)w.mom, w.st,
                   d_result);

@@ -28,6 +28,9 @@ struct Slot {
     void* d_meter_ws = nullptr;          // metering only (mgb_pipeline_enable_loudness)
     mgb_loudness_result* d_meter = nullptr;
     mgb_loudness_result* h_meter = nullptr;  // pinned
+    void* d_search_ws = nullptr;         // loudness target only (mgb_pipeline_enable_loudness_target)
+    mgb_loudness_target_report* d_report = nullptr;
+    mgb_loudness_target_report* h_report = nullptr;  // pinned
     mgb_track_layout layout;
     bool busy = false;
 #ifndef MGB_EMULATE
@@ -49,6 +52,9 @@ struct mgb_pipeline {
     bool meter = false;  // mgb_pipeline_enable_loudness
     mgb_loudness_params meter_params;
     int64_t meter_ws_bytes = 0;
+    bool target = false;  // mgb_pipeline_enable_loudness_target
+    mgb_loudness_target target_params;
+    int64_t search_ws_bytes = 0;
 #ifndef MGB_EMULATE
     cudaStream_t s_h2d = nullptr, s_compute = nullptr, s_d2h = nullptr;
 #endif
@@ -204,12 +210,16 @@ int mgb_pipeline_destroy(mgb_pipeline* p) {
         dev_free(s.d_state);
         if (s.d_meter_ws) dev_free(s.d_meter_ws);
         if (s.d_meter) dev_free(s.d_meter);
+        if (s.d_search_ws) dev_free(s.d_search_ws);
+        if (s.d_report) dev_free(s.d_report);
 #ifdef MGB_EMULATE
         free(s.h_state);
         free(s.h_meter);
+        free(s.h_report);
 #else
         if (s.h_state) cudaFreeHost(s.h_state);
         if (s.h_meter) cudaFreeHost(s.h_meter);
+        if (s.h_report) cudaFreeHost(s.h_report);
         if (s.h2d_done) cudaEventDestroy(s.h2d_done);
         if (s.compute_done) cudaEventDestroy(s.compute_done);
         if (s.d2h_done) cudaEventDestroy(s.d2h_done);
@@ -271,6 +281,50 @@ int mgb_pipeline_wait_loudness(mgb_pipeline* p, int32_t slot, mgb_track_state* s
     return MGB_OK;
 }
 
+int mgb_pipeline_enable_loudness_target(mgb_pipeline* p, const mgb_loudness_target* target) {
+    MGB_REQUIRE(p != nullptr, MGB_ERR_INVALID, "pipeline: NULL argument");
+    MGB_REQUIRE(p->meter, MGB_ERR_INVALID, "pipeline: a loudness target needs metering (mgb_pipeline_enable_loudness) first");
+    MGB_REQUIRE(!p->submitted && !p->target, MGB_ERR_INVALID, "pipeline: a loudness target is set once, before the first submit");
+    MGB_TRY(loudness_target_validate(target, &p->meter_params));
+    MGB_REQUIRE(p->meter_params.sample_rate == p->plan.sample_rate, MGB_ERR_INVALID,
+                "pipeline: the meter's rate %d differs from the plan's %d", p->meter_params.sample_rate, p->plan.sample_rate);
+    const int64_t bytes = mgb_loudness_target_workspace_bytes(&p->meter_params, std::max<int64_t>(p->max_target, 1));
+    MGB_REQUIRE(bytes > 0, MGB_ERR_INVALID, "pipeline: bad loudness parameters");
+    for (auto& s : p->slots) {
+        s.d_search_ws = dev_alloc((size_t)bytes);
+        s.d_report = (mgb_loudness_target_report*)dev_alloc(sizeof(mgb_loudness_target_report));
+#ifdef MGB_EMULATE
+        s.h_report = (mgb_loudness_target_report*)malloc(sizeof(mgb_loudness_target_report));
+#else
+        if (cudaMallocHost((void**)&s.h_report, sizeof(mgb_loudness_target_report)) != cudaSuccess) s.h_report = nullptr;
+#endif
+        if (!s.d_search_ws || !s.d_report || !s.h_report) {
+            set_error("pipeline: allocation of the loudness-target buffers failed");
+            return MGB_ERR_CUDA;  // (what was allocated is released by mgb_pipeline_destroy)
+        }
+        memset(s.h_report, 0, sizeof(mgb_loudness_target_report));
+    }
+    p->target_params = *target;
+    p->search_ws_bytes = bytes;
+    p->target = true;
+    return MGB_OK;
+}
+
+int mgb_pipeline_wait_loudness_target(mgb_pipeline* p, int32_t slot, mgb_track_state* state_out,
+                                      mgb_loudness_result* loudness_out, mgb_loudness_target_report* report_out) {
+    MGB_REQUIRE(p && p->target, MGB_ERR_INVALID, "pipeline: no loudness target is set");
+    MGB_TRY(mgb_pipeline_wait_loudness(p, slot, state_out, loudness_out));
+    if (report_out) *report_out = *p->slots[slot].h_report;
+    return MGB_OK;
+}
+
+// Stage 4 of a submission: the limited output into d_out, at the pipeline's loudness target if it has one.
+static int submit_finalize(mgb_pipeline* p, Slot& s, void* sc) {
+    if (!p->target) return mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc);
+    return mgb_finalize_to_loudness(&p->plan, &s.layout, &p->meter_params, &p->target_params, s.d_result, s.d_out,
+                                    s.d_workspace, s.d_search_ws, p->search_ws_bytes, s.d_state, s.d_report, sc);
+}
+
 // Metering of a submission's float32 limited output, on the slot's compute stream (nothing without metering).
 static int submit_meter(mgb_pipeline* p, Slot& s, int64_t frames, void* sc) {
     if (!p->meter) return MGB_OK;
@@ -314,12 +368,13 @@ static int submit_impl(mgb_pipeline* p, const float* h_target_lr, int64_t target
     MGB_TRY(submit_levels(p, s, d_profile, sc));
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
-    MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
+    MGB_TRY(submit_finalize(p, s, sc));
     MGB_TRY(submit_meter(p, s, target_frames, sc));
 #ifdef MGB_EMULATE
     memcpy(h_out_limited, s.d_out, tb);
     memcpy(s.h_state, s.d_state, sizeof(mgb_track_state));
     if (p->meter) memcpy(s.h_meter, s.d_meter, sizeof(mgb_loudness_result));
+    if (p->target) memcpy(s.h_report, s.d_report, sizeof(mgb_loudness_target_report));
 #else
     MGB_CUDA_OK(cudaEventRecord(s.compute_done, s.compute));
     MGB_CUDA_OK(cudaStreamWaitEvent(p->s_d2h, s.compute_done, 0));
@@ -327,6 +382,9 @@ static int submit_impl(mgb_pipeline* p, const float* h_target_lr, int64_t target
     MGB_CUDA_OK(cudaMemcpyAsync(s.h_state, s.d_state, sizeof(mgb_track_state), cudaMemcpyDeviceToHost, p->s_d2h));
     if (p->meter)
         MGB_CUDA_OK(cudaMemcpyAsync(s.h_meter, s.d_meter, sizeof(mgb_loudness_result), cudaMemcpyDeviceToHost, p->s_d2h));
+    if (p->target)
+        MGB_CUDA_OK(cudaMemcpyAsync(s.h_report, s.d_report, sizeof(mgb_loudness_target_report), cudaMemcpyDeviceToHost,
+                                    p->s_d2h));
     MGB_CUDA_OK(cudaEventRecord(s.d2h_done, p->s_d2h));
 #endif
     s.busy = true;
@@ -387,13 +445,14 @@ static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t ta
     MGB_TRY(submit_levels(p, s, d_profile, sc));
     MGB_TRY(mgb_match_frequencies(&p->plan, &s.layout, s.d_target, s.d_result, nullptr, s.d_workspace, s.d_state, sc));
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
-    MGB_TRY(mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc));
+    MGB_TRY(submit_finalize(p, s, sc));
     MGB_TRY(submit_meter(p, s, target_frames, sc));  // (the float32 output, before quantisation)
     MGB_TRY(mgb_pcm_encode(s.d_out, out_bits, s.d_pcm_out, target_frames * 2, sc));
 #ifdef MGB_EMULATE
     memcpy(h_out_pcm, s.d_pcm_out, ob);
     memcpy(s.h_state, s.d_state, sizeof(mgb_track_state));
     if (p->meter) memcpy(s.h_meter, s.d_meter, sizeof(mgb_loudness_result));
+    if (p->target) memcpy(s.h_report, s.d_report, sizeof(mgb_loudness_target_report));
 #else
     MGB_CUDA_OK(cudaEventRecord(s.compute_done, s.compute));
     MGB_CUDA_OK(cudaStreamWaitEvent(p->s_d2h, s.compute_done, 0));
@@ -401,6 +460,9 @@ static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t ta
     MGB_CUDA_OK(cudaMemcpyAsync(s.h_state, s.d_state, sizeof(mgb_track_state), cudaMemcpyDeviceToHost, p->s_d2h));
     if (p->meter)
         MGB_CUDA_OK(cudaMemcpyAsync(s.h_meter, s.d_meter, sizeof(mgb_loudness_result), cudaMemcpyDeviceToHost, p->s_d2h));
+    if (p->target)
+        MGB_CUDA_OK(cudaMemcpyAsync(s.h_report, s.d_report, sizeof(mgb_loudness_target_report), cudaMemcpyDeviceToHost,
+                                    p->s_d2h));
     MGB_CUDA_OK(cudaEventRecord(s.d2h_done, p->s_d2h));
 #endif
     s.busy = true;

@@ -42,7 +42,7 @@ class Config:
                  lowess_frac: float = 0.0375, lowess_it: int = 0, lowess_delta: float = 0.001,
                  preview_size: float = 30, preview_analysis_step: float = 5, preview_fade_size: float = 1,
                  preview_fade_coefficient: float = 8, temp_folder: str = None,
-                 limiter: LimiterConfig = None, true_peak: bool = False):
+                 limiter: LimiterConfig = None, true_peak: bool = False, loudness_target: float = None):
         sr = internal_sample_rate
         _require(isinstance(sr, int) and sr > 0, "internal_sample_rate must be a positive int")
         if sr != 44100:
@@ -74,6 +74,9 @@ class Config:
             limiter = _DEFAULT_LIMITER
         _require(isinstance(limiter, LimiterConfig), "limiter must be a LimiterConfig")
         _require(isinstance(true_peak, bool), "true_peak must be a bool")
+        _require(loudness_target is None or (isinstance(loudness_target, (int, float)) and not isinstance(loudness_target, bool)
+                                             and math.isfinite(loudness_target) and -70 < loudness_target < 0),
+                 "loudness_target must be None or a finite LUFS value in (-70, 0)")
 
         self.internal_sample_rate = sr
         self.max_length = max_length
@@ -98,6 +101,9 @@ class Config:
         # True: the limiter, its early-out and the normalised output hold `threshold` on the true peak (the signal
         # between samples, through the loudness meter's interpolator) instead of the sample peak
         self.true_peak = true_peak
+        # LUFS: the limited outputs are driven into the limiter until they read this integrated loudness (a search on
+        # the device; final_amplitude_coefficient is not applied there).  None: the reference's level, as before
+        self.loudness_target = None if loudness_target is None else float(loudness_target)
 
 
 _DEFAULT_LIMITER = LimiterConfig()  # shared default instance, like the reference's default argument

@@ -185,6 +185,24 @@ class TrackSession:
                                                      self.state.data_ptr(), _stream_ptr(self.device)))
         return limited, plain, normalized
 
+    def finalize_to_loudness(self, target_lufs: float, need_no_limiter: bool, need_no_limiter_normalized: bool):
+        """finalize with the limited output searched to `target_lufs` (mgb_finalize_to_loudness); the other two
+        outputs as mgb_finalize writes them.  -> (limited, plain, normalized, the device report)"""
+        from .loudness import device_meter, target_params
+        limited, plain, normalized = self.finalize(False, need_no_limiter, need_no_limiter_normalized)
+        n = self.layout.target_frames
+        meter = device_meter(self.plan.tables.sample_rate, self.device)
+        search_bytes = int(self.lib.mgb_loudness_target_workspace_bytes(C.byref(meter.params), n))
+        search = torch.empty(search_bytes, dtype=torch.uint8, device=self.device)
+        report = torch.empty(C.sizeof(_native.LoudnessTargetReport), dtype=torch.uint8, device=self.device)
+        limited = torch.empty((n, 2), dtype=torch.float32, device=self.device)
+        p, l = self._args()
+        _native.check(self.lib, self.lib.mgb_finalize_to_loudness(
+            p, l, C.byref(meter.params), C.byref(target_params(target_lufs)), self.result.data_ptr(), limited.data_ptr(),
+            self.workspace.data_ptr(), search.data_ptr(), search_bytes, self.state.data_ptr(), report.data_ptr(),
+            _stream_ptr(self.device)))
+        return limited, plain, normalized, report
+
     def read_state(self) -> _native.TrackState:
         """One device->host read of the job's scalars (synchronises)."""
         raw = self.state.cpu().numpy().tobytes()

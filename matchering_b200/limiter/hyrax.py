@@ -16,12 +16,16 @@ from ..plan import limiter_constants
 
 def limit(array, config: Config):
     """Returns the limited (N, 2) array; like the reference, returns `array` ITSELF (same object)
-    when no frame exceeds the threshold (hyrax.py:83-85)."""
+    when no frame exceeds the threshold (hyrax.py:83-85).  With Config(loudness_target=T) the input is driven into the
+    limiter until the output reads T LUFS (a new array, always)."""
     _require_cuda()
     lib = _native.load()
     params = limiter_params(limiter_constants(config))
     device = torch.device("cuda", torch.cuda.current_device())
     debug("The limiter is started. Preparing the gain envelope...")
+    if config.loudness_target is not None:
+        out, _ = limit_to_loudness(array, config)
+        return out
     if host_array_ok(array):
         return _limit_host(array, params, device, lib)
     with torch.cuda.device(device):
@@ -79,3 +83,31 @@ def _limit_host(array: np.ndarray, params, device, lib):
         debug("The limiter is not needed!")
         return array
     return out
+
+
+def limit_to_loudness(array, config: Config):
+    """limit() at Config.loudness_target (mgb_limit_to_loudness).  -> (output in the caller's array type, LoudnessTarget)"""
+    from ..loudness import LoudnessTarget, debug_target, device_meter, target_params
+    _require_cuda()
+    lib = _native.load()
+    params = limiter_params(limiter_constants(config))
+    device = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+        x = to_device_f32(array, device)
+        frames = x.shape[0]
+        if frames <= 6:
+            raise ValueError("The length of the input vector x must be greater than padlen, which is 6.")
+        meter = device_meter(config.internal_sample_rate, device)
+        ws_bytes = int(lib.mgb_limiter_workspace_bytes(C.byref(params), frames)) + int(
+            lib.mgb_loudness_target_workspace_bytes(C.byref(meter.params), frames))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        out = torch.empty_like(x)
+        report = torch.empty(C.sizeof(_native.LoudnessTargetReport), dtype=torch.uint8, device=device)
+        _native.check(lib, lib.mgb_limit_to_loudness(C.byref(params), C.byref(meter.params),
+                                                     C.byref(target_params(config.loudness_target)), x.data_ptr(),
+                                                     out.data_ptr(), frames, ws.data_ptr(), ws_bytes, report.data_ptr(),
+                                                     _stream_ptr(device)))
+        t = LoudnessTarget.from_report(config.loudness_target,
+                                       _native.LoudnessTargetReport.from_buffer_copy(report.cpu().numpy().tobytes()))
+        debug_target(t)
+        return to_host_like(out, array), t

@@ -43,6 +43,48 @@ class Loudness:
                    db(max(r.sample_peak[0], r.sample_peak[1])), max(tp), tp)
 
 
+# the largest drive a loudness target may apply on top of the correction gain (Config(loudness_target=...)), dB
+LOUDNESS_TARGET_MAX_GAIN_DB = 24.0
+
+_TARGET_STATUS = {_native.MGB_LOUDNESS_REACHED: "reached", _native.MGB_LOUDNESS_UNREACHABLE: "unreachable",
+                  _native.MGB_LOUDNESS_BRACKET: "bracket", _native.MGB_LOUDNESS_PASSES: "passes",
+                  _native.MGB_LOUDNESS_UNDEFINED: "undefined"}
+
+
+@dataclass(frozen=True)
+class LoudnessTarget:
+    """How a loudness-targeted limiter run ended (Config(loudness_target=...)).  gain_db is the drive into the limiter on
+    top of the correction gain, integrated the loudness measured on the samples written; status is "reached" (within
+    0.01 LU), "unreachable" (still too quiet at the largest drive), "bracket" (the loudness jumps across the target within
+    1e-3 dB), "passes" (the pass limit came first) or "undefined" (silence, or shorter than one 400 ms window)."""
+    target: float
+    gain_db: float
+    integrated: float
+    input_integrated: float
+    passes: int
+    status: str
+    trace: tuple  # ((gain_db, integrated), ...) per pass
+
+    @classmethod
+    def from_report(cls, target: float, r: _native.LoudnessTargetReport) -> "LoudnessTarget":
+        n = int(r.passes)
+        return cls(float(target), float(r.gain_db), float(r.integrated), float(r.input_integrated), n,
+                   _TARGET_STATUS.get(int(r.status), f"status {int(r.status)}"),
+                   tuple((float(r.trace_gain_db[k]), float(r.trace_integrated[k])) for k in range(n)))
+
+
+def target_params(target_lufs: float) -> _native.LoudnessTargetParams:
+    t = _native.LoudnessTargetParams()
+    t.target_lufs, t.max_gain_db = float(target_lufs), LOUDNESS_TARGET_MAX_GAIN_DB
+    return t
+
+
+def debug_target(t: LoudnessTarget) -> None:
+    from .log import debug
+    debug(f"Loudness target {t.target:.2f} LUFS: drive {t.gain_db:+.4f} dB, measured {t.integrated:.4f} LUFS "
+          f"after {t.passes} pass(es), {t.status}")
+
+
 class DeviceMeter:
     """The C parameters of one rate, with their filter tables on one device (cached per device and rate)."""
 

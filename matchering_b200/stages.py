@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import torch
 
+from . import _native
 from .defaults import Config
 from .engine import (TrackSession, get_plan, host_array_ok, stages_main_host, stages_main_host_profiled, to_device_f32,
                      to_host_like)
@@ -29,7 +30,8 @@ def main(target, reference, config: Config, need_default: bool = True, need_no_l
     profiled = isinstance(reference, ReferenceProfile)
     if profiled:
         reference.check_config(config)
-    if host_array_ok(target) and (profiled or host_array_ok(reference)):
+    # (a loudness target runs its search in the device session below; the single-call host entry has no target)
+    if host_array_ok(target) and (profiled or host_array_ok(reference)) and config.loudness_target is None:
         plan = get_plan(config)
         with torch.cuda.device(plan.device):
             debug_line()
@@ -110,9 +112,19 @@ def main_device(target, reference, config: Config, need_default: bool = True, ne
 
         debug_line()
         info(Code.INFO_FINALIZING)               # stages.py:182
-        limited, plain, normalized = session.finalize(need_default, need_no_limiter, need_no_limiter_normalized)
+        report = None
+        if need_default and config.loudness_target is not None:
+            limited, plain, normalized, report = session.finalize_to_loudness(config.loudness_target, need_no_limiter,
+                                                                              need_no_limiter_normalized)
+        else:
+            limited, plain, normalized = session.finalize(need_default, need_no_limiter, need_no_limiter_normalized)
 
         if debug_enabled():  # one read-back of the device scalars, only when somebody listens
             _debug_scalars(session.read_state(), session.layout, reference if profiled else None)
+            if report is not None:
+                from .loudness import LoudnessTarget, debug_target
+                raw = report.cpu().numpy().tobytes()
+                debug_target(LoudnessTarget.from_report(config.loudness_target,
+                                                        _native.LoudnessTargetReport.from_buffer_copy(raw)))
 
     return limited, plain, normalized
