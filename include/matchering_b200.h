@@ -522,6 +522,35 @@ int mgb_convert_f32_to_f64(const float* d_in, double* d_out, int64_t count, void
 int mgb_pcm_decode(const void* d_pcm, int32_t bits, float* d_out, int64_t count, void* stream);
 int mgb_pcm_encode(const float* d_in, int32_t bits, void* d_pcm, int64_t count, void* stream);
 
+/* Dithered PCM encode: TPDF dither, optionally noise-shaped by error feedback, then rounding to 16 or 24 bits, in place
+ * of mgb_pcm_encode's plain rounding (DESIGN.md §4 "Dither" states the definition the output follows to the bit).  Per
+ * channel of the stereo float32 frames at d_lr, in float64, top = 2^(bits-1) - 1:
+ *   d[n, c] = (a - b) / 2^24, a = z >> 40, b = (z >> 16) & 0xFFFFFF, z = splitmix64 finaliser of
+ *             seed + (2n + c + 1) * 0x9E3779B97F4A7C15 (mod 2^64)                TPDF in (-1, 1) LSB
+ *   fb = sum of h[k-1] * e[n-k] for k = taps .. 1, oldest first, every product and sum rounded (no FMA)
+ *   v = x * top - fb, q = rint(v + d) (ties to even), e[n] = q - v, out = clip(q, -top - 1, top)
+ *   (a non-finite q: e[n] = 0 and mgb_pcm_encode's sample)
+ * Each channel runs in segments of 1024 frames, each from a zero error history 32 frames before its first frame (at
+ * frame 0 for the first), so the output depends on neither the grid nor the stream.  |e| < 1.5 LSB for any taps.
+ * taps = 0 is flat TPDF.  Zero taps appended to h change no bit.  d_pcm: int16 pairs or packed little-endian 24-bit
+ * triplets, `frames` frames.  MGB_ERR_UNSUPPORTED for bits other than 16 / 24; MGB_ERR_INVALID for taps outside
+ * [0, MGB_MAX_DITHER_TAPS], a non-finite h[0 .. taps), a nonzero `reserved`, NULL or not 16-byte aligned pointers, or
+ * frames < 0.  frames = 0 does nothing.  No workspace. */
+#define MGB_MAX_DITHER_TAPS 32
+typedef struct mgb_dither_params {
+    uint64_t seed;
+    int32_t taps;     /* shaping taps h_1 .. h_taps in h[0 .. taps) */
+    int32_t reserved; /* 0 */
+    double h[MGB_MAX_DITHER_TAPS];
+} mgb_dither_params;
+int mgb_pcm_encode_dithered(const mgb_dither_params* params, const float* d_lr, int64_t frames, int32_t bits, void* d_pcm,
+                            void* stream);
+/* The batch pipeline (above): dither every later PCM submission.  Its limited output is then quantised by
+ * mgb_pcm_encode_dithered with these parameters instead of mgb_pcm_encode; float32 submissions are unaffected.  Called
+ * once, before the first submit; MGB_ERR_INVALID otherwise, or for parameters mgb_pcm_encode_dithered would reject.  A
+ * pipeline that never calls this runs exactly what it did before. */
+int mgb_pipeline_enable_dither(mgb_pipeline* p, const mgb_dither_params* params);
+
 /* Checker reductions on the device (matchering/checker.py:64-88,140-142; dsp.count_max_peaks
  * dsp.py:49-54).  mgb_check_peaks: d_scratch16 (16 bytes, device) receives {float peak; pad;
  * uint64 count of samples with isclose(|x|, peak)} for `frames` stereo frames.

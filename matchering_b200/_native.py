@@ -52,6 +52,18 @@ class LimiterParams(C.Structure):
         return p
 
 
+MGB_MAX_DITHER_TAPS = 32
+
+
+class DitherParams(C.Structure):
+    _fields_ = [
+        ("seed", C.c_uint64),
+        ("taps", C.c_int32),
+        ("reserved", C.c_int32),
+        ("h", C.c_double * MGB_MAX_DITHER_TAPS),
+    ]
+
+
 class Plan(C.Structure):
     _fields_ = [
         ("sample_rate", C.c_int32),
@@ -270,6 +282,8 @@ PROTOTYPES = {
     "mgb_convert_f32_to_f64": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "mgb_pcm_decode": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "mgb_pcm_encode": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mgb_pcm_encode_dithered": (C.c_int, [C.POINTER(DitherParams), C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
+    "mgb_pipeline_enable_dither": (C.c_int, [C.c_void_p, C.POINTER(DitherParams)]),
     "mgb_check_peaks": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "mgb_window_energy": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
     "mgb_preview_piece": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_int64, C.c_void_p]),

@@ -21,13 +21,15 @@ from .profile import ReferenceProfile
 
 class MasteringPipeline:
     def __init__(self, config, max_target_frames: int, max_reference_frames: int, depth: int = 3, device=None,
-                 loudness: bool = False):
+                 loudness: bool = False, dither: str = None, dither_seed: int = 0):
         """max_reference_frames bounds the references submitted as samples; profiles have no such bound
         (a pipeline that only takes profiles may pass smallest_reference_frames(config)).
         loudness=True meters every limited output on the device (mg.loudness's meter, at the Config's rate)
         and `wait_loudness` returns it.  With Config(loudness_target=T) every limited output is driven to T LUFS
         (mgb_pipeline_enable_loudness_target; its search uses the meter, which is then always on) and
-        `wait_loudness_target` returns the meter and the search's report."""
+        `wait_loudness_target` returns the meter and the search's report.
+        dither ("tpdf" or "shaped", as in mg.Result) dithers every `submit_pcm` result with dither_seed
+        (mgb_pipeline_enable_dither); float32 submissions are unaffected."""
         self.config = config
         self.plan = get_plan(config, device)
         self.lib = self.plan.lib
@@ -39,6 +41,10 @@ class MasteringPipeline:
         self._meter = (device_meter(config.internal_sample_rate, self.device)
                        if loudness or self.target is not None else None)
         self._pending = {}  # slot -> (target, reference, out) kept alive until the slot is waited on
+        dither_params = None
+        if dither is not None:
+            from .dither import params
+            dither_params = params(dither, config.internal_sample_rate, dither_seed)
         with torch.cuda.device(self.device):
             _native.check(self.lib, self.lib.mgb_pipeline_create(C.byref(self.plan.struct), max_target_frames,
                                                                  max_reference_frames, depth, C.byref(self._handle)))
@@ -46,6 +52,11 @@ class MasteringPipeline:
                 status = self.lib.mgb_pipeline_enable_loudness(self._handle, C.byref(self._meter.params))
                 if status == _native.MGB_OK and self.target is not None:
                     status = self.lib.mgb_pipeline_enable_loudness_target(self._handle, C.byref(target_params(self.target)))
+                if status != _native.MGB_OK:
+                    self.close()
+                    _native.check(self.lib, status)
+            if dither_params is not None:
+                status = self.lib.mgb_pipeline_enable_dither(self._handle, C.byref(dither_params))
                 if status != _native.MGB_OK:
                     self.close()
                     _native.check(self.lib, status)

@@ -72,15 +72,22 @@ def process(target: str, reference, results: list, config: Config = None,
 def _export(wanted: Result, audio, sample_rate: int, name: str = "result") -> None:
     """16/24-bit WAV results are quantised on the device and written as they come back (a quarter of
     the device->host bytes of a float64 array); everything else takes the reference's route through
-    a host float array and `save`."""
+    a host float array and `save`.  Dithered results (Result(dither=...)) are always quantised on the device,
+    by the dithered encoder, whether or not libsndfile is present."""
     from .results import real_soundfile
     is_wav = wanted.file.lower().endswith(".wav")
-    if is_wav and wanted.subtype in ("PCM_16", "PCM_24") and real_soundfile() is None:
+    dither = getattr(wanted, "dither", None)
+    if is_wav and wanted.subtype in ("PCM_16", "PCM_24") and (dither is not None or real_soundfile() is None):
         from . import wavio
         from .engine import encode_pcm
         bits = int(wanted.subtype[4:])
+        params = None
+        if dither is not None:
+            from .dither import params as dither_params
+            params = dither_params(dither, sample_rate, wanted.dither_seed)
+            debug(f"Dither: {dither}, seed {wanted.dither_seed}")
         debug(f"Saving the {name.upper()} {sample_rate} Hz Stereo {wanted.subtype} to: '{wanted.file}'...")
-        wavio.write_pcm(wanted.file, encode_pcm(audio, bits), sample_rate, bits)
+        wavio.write_pcm(wanted.file, encode_pcm(audio, bits, params), sample_rate, bits)
         debug(f"'{wanted.file}' is saved")
     else:
         save(wanted.file, audio.cpu().numpy().astype("float64"), sample_rate, wanted.subtype, name)

@@ -881,6 +881,17 @@ int mgb_pcm_encode(const float* d_in, int32_t bits, void* d_pcm, int64_t count, 
     return launch_pcm_encode(d_in, bits, d_pcm, count, (cudaStream_t)stream);
 }
 
+int mgb_pcm_encode_dithered(const mgb_dither_params* params, const float* d_lr, int64_t frames, int32_t bits, void* d_pcm,
+                            void* stream) {
+    MGB_TRY(dither_validate(params));
+    MGB_REQUIRE(bits == 16 || bits == 24, MGB_ERR_UNSUPPORTED, "pcm_encode_dithered: %d-bit samples (16 and 24)", bits);
+    MGB_TRY(check_aligned(d_lr, "d_lr"));
+    MGB_TRY(check_aligned(d_pcm, "d_pcm"));
+    MGB_REQUIRE(frames >= 0, MGB_ERR_INVALID, "pcm_encode_dithered: %lld frames", (long long)frames);
+    if (frames == 0) return MGB_OK;
+    return launch_pcm_encode_dithered(*params, d_lr, frames, bits, d_pcm, (cudaStream_t)stream);
+}
+
 int mgb_check_peaks(const float* d_lr, int64_t frames, void* d_scratch16, void* stream) {
     MGB_REQUIRE(d_lr && d_scratch16 && frames > 0, MGB_ERR_INVALID, "check_peaks: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;

@@ -302,6 +302,12 @@ unsigned grid_for(long long items, int per_block) {
 
 }  // namespace
 
+}  // namespace mgb
+
+#include "dither.cuh"  // dithered PCM encode (mgb_pcm_encode_dithered)
+
+namespace mgb {
+
 int launch_loud_sumsq(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws, int step,
                       mgb_track_state* state, cudaStream_t stream) {
     // The grid is fixed before the device decides between list and result, so it is sized for a pass over
@@ -367,6 +373,47 @@ int launch_pcm_encode(const float* in, int bits, void* out, int64_t count, cudaS
         return launch("pcm24_encode_kernel", pcm24_encode_kernel, dim3(grid_for(count, 1024)), dim3(256), 0, stream, in,
                       (unsigned char*)out, (long long)count);
     set_error("pcm encode: %d-bit samples have no kernel (16 and 24 do)", bits);
+    return MGB_ERR_UNSUPPORTED;
+}
+
+namespace {
+template <int BITS, int K>
+int launch_dither_instance(const char* what, const DitherArgs& args, const float* in, int64_t frames, void* out,
+                           cudaStream_t stream) {
+    const long long segments = (frames + kDitherSegment - 1) / kDitherSegment;
+    return launch(what, pcm_dither_encode_kernel<BITS, K>, dim3((unsigned)((segments + kDitherSegs - 1) / kDitherSegs)),
+                  dim3(kDitherThreads), 0, stream, args, (const float2*)in, (long long)frames, (unsigned char*)out);
+}
+}  // namespace
+
+int dither_validate(const mgb_dither_params* p) {
+    MGB_REQUIRE(p != nullptr, MGB_ERR_INVALID, "dither: params is NULL");
+    MGB_REQUIRE(p->taps >= 0 && p->taps <= MGB_MAX_DITHER_TAPS, MGB_ERR_INVALID, "dither: %d taps (0 .. %d)", p->taps,
+                MGB_MAX_DITHER_TAPS);
+    MGB_REQUIRE(p->reserved == 0, MGB_ERR_INVALID, "dither: reserved must be 0");
+    for (int k = 0; k < p->taps; ++k) MGB_REQUIRE(isfinite(p->h[k]), MGB_ERR_INVALID, "dither: tap h[%d] is not finite", k);
+    return MGB_OK;
+}
+
+// Instances: K = 0 (flat TPDF), 12 (the length of the shaped filter dither.py designs) and MGB_MAX_DITHER_TAPS;
+// a shorter filter runs on the next instance up with its taps zero-padded, which changes no bit.
+int launch_pcm_encode_dithered(const mgb_dither_params& p, const float* in, int64_t frames, int bits, void* out,
+                               cudaStream_t stream) {
+    DitherArgs args;
+    args.seed = (unsigned long long)p.seed;
+    for (int k = 0; k < MGB_MAX_DITHER_TAPS; ++k) args.h[k] = k < p.taps ? p.h[k] : 0.0;
+    const int K = p.taps == 0 ? 0 : p.taps <= 12 ? 12 : MGB_MAX_DITHER_TAPS;
+    if (bits == 16) {
+        if (K == 0) return launch_dither_instance<16, 0>("pcm_dither_encode_kernel<16,0>", args, in, frames, out, stream);
+        if (K == 12) return launch_dither_instance<16, 12>("pcm_dither_encode_kernel<16,12>", args, in, frames, out, stream);
+        return launch_dither_instance<16, MGB_MAX_DITHER_TAPS>("pcm_dither_encode_kernel<16,32>", args, in, frames, out, stream);
+    }
+    if (bits == 24) {
+        if (K == 0) return launch_dither_instance<24, 0>("pcm_dither_encode_kernel<24,0>", args, in, frames, out, stream);
+        if (K == 12) return launch_dither_instance<24, 12>("pcm_dither_encode_kernel<24,12>", args, in, frames, out, stream);
+        return launch_dither_instance<24, MGB_MAX_DITHER_TAPS>("pcm_dither_encode_kernel<24,32>", args, in, frames, out, stream);
+    }
+    set_error("pcm encode: %d-bit samples have no dithered kernel (16 and 24 do)", bits);
     return MGB_ERR_UNSUPPORTED;
 }
 

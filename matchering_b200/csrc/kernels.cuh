@@ -149,6 +149,9 @@ int launch_window_energy(const float2* x, int64_t window, int64_t step, int coun
 int launch_preview_piece(const float2* in, float2* out, int64_t frames, float clip_to, int64_t fade, cudaStream_t stream);
 int launch_pcm_decode(const void* in, int bits, float* out, int64_t count, cudaStream_t stream);
 int launch_pcm_encode(const float* in, int bits, void* out, int64_t count, cudaStream_t stream);
+int dither_validate(const mgb_dither_params* p);  // MGB_ERR_INVALID for parameters the dithered encoder rejects
+int launch_pcm_encode_dithered(const mgb_dither_params& p, const float* in, int64_t frames, int bits, void* out,
+                               cudaStream_t stream);
 int launch_convert_f64_f32(const double* in, float* out, int64_t count, cudaStream_t stream);
 int launch_convert_f32_f64(const float* in, double* out, int64_t count, cudaStream_t stream);
 

@@ -55,6 +55,8 @@ struct mgb_pipeline {
     bool target = false;  // mgb_pipeline_enable_loudness_target
     mgb_loudness_target target_params;
     int64_t search_ws_bytes = 0;
+    bool dither = false;  // mgb_pipeline_enable_dither
+    mgb_dither_params dither_params;
 #ifndef MGB_EMULATE
     cudaStream_t s_h2d = nullptr, s_compute = nullptr, s_d2h = nullptr;
 #endif
@@ -318,6 +320,15 @@ int mgb_pipeline_wait_loudness_target(mgb_pipeline* p, int32_t slot, mgb_track_s
     return MGB_OK;
 }
 
+int mgb_pipeline_enable_dither(mgb_pipeline* p, const mgb_dither_params* params) {
+    MGB_REQUIRE(p != nullptr, MGB_ERR_INVALID, "pipeline: NULL argument");
+    MGB_REQUIRE(!p->submitted && !p->dither, MGB_ERR_INVALID, "pipeline: dither is enabled once, before the first submit");
+    MGB_TRY(dither_validate(params));
+    p->dither_params = *params;
+    p->dither = true;
+    return MGB_OK;
+}
+
 // Stage 4 of a submission: the limited output into d_out, at the pipeline's loudness target if it has one.
 static int submit_finalize(mgb_pipeline* p, Slot& s, void* sc) {
     if (!p->target) return mgb_finalize(&p->plan, &s.layout, s.d_result, s.d_out, nullptr, nullptr, s.d_workspace, s.d_state, sc);
@@ -447,7 +458,10 @@ static int submit_pcm_impl(mgb_pipeline* p, const void* h_target_pcm, int32_t ta
     MGB_TRY(mgb_correct_levels(&p->plan, &s.layout, s.d_workspace, s.d_state, sc));
     MGB_TRY(submit_finalize(p, s, sc));
     MGB_TRY(submit_meter(p, s, target_frames, sc));  // (the float32 output, before quantisation)
-    MGB_TRY(mgb_pcm_encode(s.d_out, out_bits, s.d_pcm_out, target_frames * 2, sc));
+    if (p->dither)
+        MGB_TRY(mgb_pcm_encode_dithered(&p->dither_params, s.d_out, target_frames, out_bits, s.d_pcm_out, sc));
+    else
+        MGB_TRY(mgb_pcm_encode(s.d_out, out_bits, s.d_pcm_out, target_frames * 2, sc));
 #ifdef MGB_EMULATE
     memcpy(h_out_pcm, s.d_pcm_out, ob);
     memcpy(s.h_state, s.d_state, sizeof(mgb_track_state));

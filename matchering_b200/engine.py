@@ -388,10 +388,11 @@ def stages_main_host_profiled(plan: DevicePlan, target: np.ndarray, profile, nee
     return tuple(outs), state
 
 
-def encode_pcm(t: torch.Tensor, bits: int):
+def encode_pcm(t: torch.Tensor, bits: int, dither: _native.DitherParams | None = None):
     """float32 CUDA (frames, 2) -> host numpy PCM: int16 (frames, 2) or packed 24-bit uint8 (frames, 6),
     quantised on the device (lrint(x * (2^(bits-1) - 1)), clipped: libsndfile's float -> int write) and
-    copied into pooled pinned memory."""
+    copied into pooled pinned memory.  With `dither` (dither.params) the dithered encoder quantises instead
+    (mgb_pcm_encode_dithered)."""
     lib = _native.load()
     frames = t.shape[0]
     if bits == 16:
@@ -400,7 +401,14 @@ def encode_pcm(t: torch.Tensor, bits: int):
         out = torch.empty((frames, 6), dtype=torch.uint8, device=t.device)
     else:
         raise ValueError("PCM width must be 16 or 24")
-    _native.check(lib, lib.mgb_pcm_encode(t.data_ptr(), bits, out.data_ptr(), frames * 2, _stream_ptr(t.device)))
+    if dither is None:
+        _native.check(lib, lib.mgb_pcm_encode(t.data_ptr(), bits, out.data_ptr(), frames * 2, _stream_ptr(t.device)))
+    else:
+        t = t.contiguous()
+        if t.data_ptr() % 16:  # (the dithered encoder takes 16-byte aligned buffers)
+            t = t.clone()
+        _native.check(lib, lib.mgb_pcm_encode_dithered(C.byref(dither), t.data_ptr(), frames, bits, out.data_ptr(),
+                                                       _stream_ptr(t.device)))
     host = HostIO.get().pool.array(tuple(out.shape), np.int16 if bits == 16 else np.uint8)
     torch.from_numpy(host).copy_(out)
     return host

@@ -27,21 +27,35 @@ def _check_format(ext: str, subtype: str = None) -> bool:
 
 
 class Result:
-    def __init__(self, file: str, subtype: str, use_limiter: bool = True, normalize: bool = True):
+    """dither: None (plain rounding, libsndfile's), "tpdf" (flat TPDF dither) or "shaped" (TPDF dither, noise-shaped
+    by dither.shaping_filter at the Config's internal rate), for 16- and 24-bit WAV results only; dither_seed selects
+    the dither's noise (the same seed gives the same file)."""
+
+    def __init__(self, file: str, subtype: str, use_limiter: bool = True, normalize: bool = True, dither: str = None,
+                 dither_seed: int = 0):
         ext = os.path.splitext(file)[1][1:].upper()
         if not _check_format(ext):
             raise TypeError(f"{ext} format is not supported")
         if not _check_format(ext, subtype):
             raise TypeError(f"{ext} format does not have {subtype} subtype")
+        if dither is not None:
+            from .dither import check_kind
+            check_kind(dither)
+            if ext != "WAV" or subtype not in ("PCM_16", "PCM_24"):
+                raise ValueError(f"dither applies to 16- and 24-bit WAV results, not {ext} {subtype}")
+            if isinstance(dither_seed, bool) or not isinstance(dither_seed, int) or not 0 <= dither_seed < 2 ** 64:
+                raise ValueError(f"dither_seed must be an integer in [0, 2^64), not {dither_seed!r}")
         self.file = file
         self.subtype = subtype
         self.use_limiter = use_limiter
         self.normalize = normalize
+        self.dither = dither
+        self.dither_seed = dither_seed
 
 
-def pcm16(file: str) -> Result:
-    return Result(file, "PCM_16")
+def pcm16(file: str, dither: str = None, dither_seed: int = 0) -> Result:
+    return Result(file, "PCM_16", dither=dither, dither_seed=dither_seed)
 
 
-def pcm24(file: str) -> Result:
-    return Result(file, "PCM_24")
+def pcm24(file: str, dither: str = None, dither_seed: int = 0) -> Result:
+    return Result(file, "PCM_24", dither=dither, dither_seed=dither_seed)
