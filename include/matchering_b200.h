@@ -121,6 +121,13 @@ typedef struct mgb_plan {
      * latency-bound CTAs). */
     const double* d_smooth_op;
     const int32_t* d_smooth_op_rows; /* [n_lin][4]: offset, first column, count, 0 */
+    /* native-rate plans only (mgb_match_frequencies_native; NULL in every other plan): how the native FIR's curve s'[j],
+     * j = 0 .. n_lin-1 at frequencies j * sample_rate / fft_size, samples the analysis plan's smoothed curve s
+     * (matchering_b200/plan.py native_tables).  Up to the edge f_e = 0.9 * R/2 of the analysis rate R,
+     * s'[j] = s[i] + w (s[i+1] - s[i]) with i = d_native_idx[j], w = d_native_w[j]; above it d_native_idx[j] = -1 and
+     * d_native_w[j] = t, the crossfade position (1 from R/2 on).  Entry n_lin is the edge itself, g_e = s(f_e). */
+    const int32_t* d_native_idx; /* [n_lin + 1] */
+    const double* d_native_w;    /* [n_lin + 1] */
 } mgb_plan;
 
 /* Per-track scalars, resident in device memory (one struct per track in flight). */
@@ -272,6 +279,28 @@ int mgb_match_levels_profiled(const mgb_plan* plan, const mgb_track_layout* layo
 int mgb_match_frequencies(const mgb_plan* plan, const mgb_track_layout* layout, const float* d_target_lr,
                           float* d_result_lr, double* d_fir_out, void* d_workspace, mgb_track_state* d_state,
                           void* stream);
+/* The FIR design of mgb_match_frequencies without its convolution: the level statistics into *d_state, the mid and
+ * side FIRs' spectra and the smoothed matching curves into the workspace.  mgb_match_frequencies is this call followed
+ * by the convolution. */
+int mgb_design_frequencies(const mgb_plan* plan, const mgb_track_layout* layout, double* d_fir_out, void* d_workspace,
+                           mgb_track_state* d_state, void* stream);
+
+/* ---- native-rate masters: stages 2-4 at the target's own rate R' (DESIGN.md section 4) -----------------------------
+ * The analysis job (plan, layout, d_workspace, d_state at the internal rate R) has run stage 1 and
+ * mgb_design_frequencies on the target resampled to R.  This call carries its smoothed curves to the FIR of
+ * native_plan (rate R', fft_size F' = F * 2^round(log2(R'/R)), with the d_native_* tables for R, F and R'), folds c0
+ * into that FIR's spectra, and convolves the native target (native_layout->target_frames frames at R') into
+ * d_native_result.  *d_native_state starts as a copy of *d_state (c0, the reference's match RMS, the final amplitude
+ * coefficient); the native FIR's peaks and the native target's peak choose the convolution's precision.  After it,
+ * mgb_correct_levels, mgb_finalize and mgb_finalize_to_loudness take native_plan, native_layout, d_native_workspace
+ * and d_native_state as they are.  native_layout is a profiled layout (mgb_track_layout_init_profiled) of
+ * native_plan.  MGB_ERR_INVALID: equal rates, an F' that does not follow from the rates, missing tables, a paired
+ * native layout; MGB_ERR_UNSUPPORTED: F' outside 512 .. 16384.
+ * d_fir_out (optional): [2][F'] doubles, the native mid and side FIRs. */
+int mgb_match_frequencies_native(const mgb_plan* plan, const mgb_track_layout* layout, const void* d_workspace,
+                                 const mgb_track_state* d_state, const mgb_plan* native_plan,
+                                 const mgb_track_layout* native_layout, const float* d_native_target, float* d_native_result,
+                                 double* d_fir_out, void* d_native_workspace, mgb_track_state* d_native_state, void* stream);
 
 /* ---- stage 3: stages.__correct_levels (stages.py:138-170) -----------------------------------
  * rms_correction_steps iterations of clip -> per-piece RMS -> loudest mask -> coefficient.  The

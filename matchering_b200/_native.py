@@ -90,6 +90,7 @@ class Plan(C.Structure):
         ("d_tw_f64_F", C.c_void_p), ("d_tw_f64_2F", C.c_void_p),
         ("d_limiter_tables", C.c_void_p),
         ("d_smooth_op", C.c_void_p), ("d_smooth_op_rows", C.c_void_p),
+        ("d_native_idx", C.c_void_p), ("d_native_w", C.c_void_p),
     ]
 
 
@@ -230,6 +231,11 @@ PROTOTYPES = {
                                                    C.c_int32, C.POINTER(C.c_int32)]),
     "mgb_match_frequencies": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mgb_design_frequencies": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]),
+    "mgb_match_frequencies_native": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p,
+                                               C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_correct_levels": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_finalize": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -34,9 +34,11 @@ def peak_warning(peak: float, hits: int, config: Config):
     return None
 
 
-def check(array: np.ndarray, sample_rate: int, config: Config, name: str):
+def check(array: np.ndarray, sample_rate: int, config: Config, name: str, native: bool = False):
     """matchering/checker.py:90-137, in the reference's order: length at the SOURCE rate (minimum
-    scaled by the rate ratio, :99), channels, resampling, then (target only) clipping / limiter."""
+    scaled by the rate ratio, :99), channels, resampling, then (target only) clipping / limiter.
+    native (the target of a Config(native_rate=True) job): -> (array, sample_rate, the stereo signal at its own
+    rate), and a resampled target is only its analysis copy, which is logged, not warned about."""
     name = name.upper()
     is_target = name == "TARGET"
     frames, channels = array.shape[0], array.shape[1]
@@ -53,17 +55,26 @@ def check(array: np.ndarray, sample_rate: int, config: Config, name: str):
     elif channels != 2:
         raise ModuleError(Code.ERROR_TARGET_NUM_OF_CHANNELS_IS_EXCEEDED if is_target
                           else Code.ERROR_REFERENCE_NUM_OF_CHANNELS_IS_EXCEEDED)
+    source = array
     if sample_rate != config.internal_sample_rate:
         debug(f"Resampling {name} audio from {sample_rate} Hz to {config.internal_sample_rate} Hz...")
         array = _resample(array, sample_rate, config.internal_sample_rate)
+        if native:
+            debug(resampled_for_analysis(sample_rate, config))
+        else:
+            (warning if is_target else info)(
+                Code.WARNING_TARGET_IS_RESAMPLED if is_target else Code.INFO_REFERENCE_IS_RESAMPLED)
         sample_rate = config.internal_sample_rate
-        (warning if is_target else info)(
-            Code.WARNING_TARGET_IS_RESAMPLED if is_target else Code.INFO_REFERENCE_IS_RESAMPLED)
     if is_target:
         code = peak_warning(*_count_max_peaks(array), config)
         if code is not None:
             warning(code)
-    return array, sample_rate
+    return (array, sample_rate, source) if native else (array, sample_rate)
+
+
+def resampled_for_analysis(rate: int, config: Config) -> str:
+    return (f"Only the TARGET's analysis copy was resampled to {config.internal_sample_rate} Hz: "
+            f"the TARGET is mastered at its own {rate} Hz")
 
 
 def check_equality(target: np.ndarray, reference: np.ndarray) -> None:

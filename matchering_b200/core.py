@@ -29,11 +29,13 @@ def process(target: str, reference, results: list, config: Config = None,
         raise RuntimeError("The result list is empty")
     temp_folder = config.temp_folder if config.temp_folder else get_temp_folder(results)
 
+    # native_rate: the target as loaded (stereo, at its own rate), for stages 2-4 when that rate is not the internal one
+    native_audio, native_rate = None, config.internal_sample_rate
     if isinstance(reference, ReferenceProfile):
         # the reference was loaded, checked and analysed when the profile was made; only its fingerprint is
         # compared with this Config here.  There are no reference samples to compare the target with.
         reference.check_config(config)
-        target_audio, target_rate = _load_and_check(target, "target", temp_folder, config)
+        target_audio, target_rate, native_audio, native_rate = _load_and_check_target(target, temp_folder, config)
         if not config.allow_equality:
             debug("The REFERENCE is a profile: the check that the TARGET differs from it is skipped")
         if (target_rate != config.internal_sample_rate or target_audio.shape[1] != 2
@@ -41,7 +43,7 @@ def process(target: str, reference, results: list, config: Config = None,
             raise ModuleError(Code.ERROR_VALIDATION)
         reference_audio = reference
     else:
-        target_audio, target_rate = _load_and_check(target, "target", temp_folder, config)
+        target_audio, target_rate, native_audio, native_rate = _load_and_check_target(target, temp_folder, config)
         reference_audio, reference_rate = _load_and_check(reference, "reference", temp_folder, config)
         if not config.allow_equality:
             _check_equality_any(target_audio, reference_audio)
@@ -50,21 +52,29 @@ def process(target: str, reference, results: list, config: Config = None,
                 or not (target_audio.shape[0] > config.fft_size and reference_audio.shape[0] > config.fft_size)):
             raise ModuleError(Code.ERROR_VALIDATION)
 
-    limited, plain, normalized = main_device(
-        target_audio, reference_audio, config,
-        need_default=any(r.use_limiter for r in results),
-        need_no_limiter=any(not r.use_limiter and not r.normalize for r in results),
-        need_no_limiter_normalized=any(not r.use_limiter and r.normalize for r in results))
+    needs = dict(need_default=any(r.use_limiter for r in results),
+                 need_no_limiter=any(not r.use_limiter and not r.normalize for r in results),
+                 need_no_limiter_normalized=any(not r.use_limiter and r.normalize for r in results))
+    if native_rate != config.internal_sample_rate:
+        from .plan import native_config
+        from .stages import main_native_device
+        limited, plain, normalized = main_native_device(native_audio, native_rate, reference_audio, config,
+                                                        analysis=target_audio, **needs)
+        # results and previews at the target's rate: the preview windows keep their length in seconds
+        out_config, preview_source = native_config(config, native_rate), native_audio
+    else:
+        limited, plain, normalized = main_device(target_audio, reference_audio, config, **needs)
+        out_config, preview_source = config, target_audio
 
     debug_line()
     info(Code.INFO_EXPORTING)
     for wanted in results:
         audio = limited if wanted.use_limiter else (normalized if wanted.normalize else plain)
-        _export(wanted, audio, config.internal_sample_rate)
+        _export(wanted, audio, out_config.internal_sample_rate)
     if preview_target or preview_result:
         from .preview_creator import create_preview
         first = next(item for item in (limited, plain, normalized) if item is not None)
-        create_preview(target_audio, first, config, preview_target, preview_result)
+        create_preview(preview_source, first, out_config, preview_target, preview_result)
     debug_line()
     info(Code.INFO_COMPLETED)
 
@@ -103,6 +113,23 @@ def _load_and_check(file: str, name: str, temp_folder: str, config: Config):
         return check_on_device(audio, config, name, rate), config.internal_sample_rate
     audio, rate = load(file, name, temp_folder)
     return check(audio, rate, config, name)
+
+
+def _load_and_check_target(file: str, temp_folder: str, config: Config):
+    """-> (the target at the internal rate, that rate, the target as loaded in stereo or None, its rate).  The
+    loaded copy is kept only for Config(native_rate=True)."""
+    if not config.native_rate:
+        audio, rate = _load_and_check(file, "target", temp_folder, config)
+        return audio, rate, None, rate
+    from .device_io import check_on_device, load_to_device
+    on_device = load_to_device(file, "target", config)
+    if on_device is not None:
+        audio, rate = on_device
+        audio, native = check_on_device(audio, config, "target", rate, native=True)
+        return audio, config.internal_sample_rate, native, rate
+    audio, rate = load(file, "target", temp_folder)
+    checked, checked_rate, native = check(audio, rate, config, "target", native=True)
+    return checked, checked_rate, native, rate
 
 
 def _check_equality_any(target_audio, reference_audio) -> None:

@@ -1,6 +1,8 @@
 // C ABI of libmatchering_b200 (include/matchering_b200.h): argument checking, workspace carving,
 // stage sequencing.  No kernel lives here except the FFT test harness.
+#include <math.h>
 #include <stdarg.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -642,10 +644,73 @@ int mgb_match_frequencies(const mgb_plan* plan, const mgb_track_layout* L, const
     MGB_TRY(check_aligned(d_target_lr, "d_target_lr"));
     MGB_TRY(check_aligned(d_result_lr, "d_result_lr"));
     MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(mgb_design_frequencies(plan, L, d_fir_out, d_workspace, d_state, stream));
+    return launch_convolve(*plan, *L, (const float2*)d_target_lr, (float2*)d_result_lr,
+                           carve_workspace(*plan, *L, d_workspace), d_state, (cudaStream_t)stream);
+}
+
+int mgb_design_frequencies(const mgb_plan* plan, const mgb_track_layout* L, double* d_fir_out, void* d_workspace,
+                           mgb_track_state* d_state, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    return launch_design(*plan, *L, carve_workspace(*plan, *L, d_workspace), nullptr, d_fir_out, d_state,
+                         (cudaStream_t)stream);
+}
+
+int mgb_match_frequencies_native(const mgb_plan* plan, const mgb_track_layout* L, const void* d_workspace,
+                                 const mgb_track_state* d_state, const mgb_plan* native_plan,
+                                 const mgb_track_layout* native_L, const float* d_native_target, float* d_native_result,
+                                 double* d_fir_out, void* d_native_workspace, mgb_track_state* d_native_state,
+                                 void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_TRY(check_plan(native_plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr && native_L != nullptr && d_native_state != nullptr, MGB_ERR_INVALID,
+                "layout/state is NULL");
+    const int R = plan->sample_rate, Rn = native_plan->sample_rate;
+    MGB_REQUIRE(R > 0 && Rn > 0 && Rn != R, MGB_ERR_INVALID, "match_frequencies_native: rates %d and %d (they must differ)",
+                R, Rn);
+    const int octaves = (int)floor(log2((double)Rn / (double)R) + 0.5);
+    const double want = ldexp((double)plan->fft_size, octaves);
+    MGB_REQUIRE(want == (double)native_plan->fft_size, MGB_ERR_INVALID,
+                "match_frequencies_native: fft_size %d at %d Hz, need %.0f for fft_size %d at %d Hz", native_plan->fft_size,
+                Rn, want, plan->fft_size, R);
+    MGB_REQUIRE(native_plan->d_native_idx != nullptr && native_plan->d_native_w != nullptr, MGB_ERR_INVALID,
+                "match_frequencies_native: the native plan has no d_native_idx / d_native_w tables");
+    MGB_REQUIRE(layout_profiled(*native_L) && native_L->target_frames > native_plan->fft_size &&
+                    native_L->target_piece >= native_plan->fft_size,
+                MGB_ERR_INVALID, "match_frequencies_native: the native layout must be a profiled layout of the native plan");
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_native_target, "d_native_target"));
+    MGB_TRY(check_aligned(d_native_result, "d_native_result"));
+    MGB_TRY(check_aligned(d_native_workspace, "d_native_workspace"));
     cudaStream_t st = (cudaStream_t)stream;
-    Workspace ws = carve_workspace(*plan, *L, d_workspace);
-    MGB_TRY(launch_design(*plan, *L, ws, nullptr, d_fir_out, d_state, st));
-    return launch_convolve(*plan, *L, (const float2*)d_target_lr, (float2*)d_result_lr, ws, d_state, st);
+    const Workspace ws = carve_workspace(*plan, *L, const_cast<void*>(d_workspace));
+    const Workspace nws = carve_workspace(*native_plan, *native_L, d_native_workspace);
+    // the analysis job's scalars, with the quantities this job measures for itself cleared (the design kernel and
+    // the convolution raise them by atomic maxima)
+#ifdef MGB_EMULATE
+    memset(nws.zero_begin, 0, nws.zero_end - nws.zero_begin);
+    memset(nws.target_peak, 0, 4);
+    memcpy(d_native_state, d_state, sizeof(mgb_track_state));
+    d_native_state->conv_peak_bits = 0.0f;
+    d_native_state->fir_peak_mid_bits = 0.0f;
+    d_native_state->fir_peak_side_bits = 0.0f;
+    d_native_state->conv_precise = 0;
+#else
+    if (cudaMemsetAsync(nws.zero_begin, 0, nws.zero_end - nws.zero_begin, st) != cudaSuccess ||
+        cudaMemsetAsync(nws.target_peak, 0, 4, st) != cudaSuccess ||
+        cudaMemcpyAsync(d_native_state, d_state, sizeof(mgb_track_state), cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemsetAsync(&d_native_state->conv_peak_bits, 0, sizeof(float), st) != cudaSuccess ||
+        cudaMemsetAsync(&d_native_state->fir_peak_mid_bits, 0,
+                        offsetof(mgb_track_state, conv_precise) + sizeof(int32_t) - offsetof(mgb_track_state, fir_peak_mid_bits),
+                        st) != cudaSuccess)
+        return cuda_status("match_frequencies_native: state copy");
+#endif
+    MGB_TRY(launch_absmax((const float2*)d_native_target, native_L->target_frames, nws.target_peak, st));
+    MGB_TRY(launch_design_native(*plan, ws, *native_plan, *native_L, nws, d_fir_out, d_native_state, st));
+    return launch_convolve(*native_plan, *native_L, (const float2*)d_native_target, (float2*)d_native_result, nws,
+                           d_native_state, st);
 }
 
 int mgb_correct_levels(const mgb_plan* plan, const mgb_track_layout* L, void* d_workspace, mgb_track_state* d_state,

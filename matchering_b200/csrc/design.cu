@@ -541,6 +541,77 @@ __device__ __noinline__ void design_fft(SplitPlanes<double> planes, const cpx<do
                                            PlaneStore<SplitPlanes<double>>{planes}, true, true);
 }
 
+// Steps F-G of a design CTA: fir = ifftshift(irfft(s)) * hann from the curve s(k), k = 0 .. F/2, then the FIR's
+// spectrum bins of residue `parity` on the ovs*F grid of the convolution with c0/(ovs*F) folded in, and its peak
+// into the track state.  design_kernel passes the curve it smoothed; design_native_kernel passes the analysis job's
+// curve carried over to its own grid.  Contains barriers.
+template <int F, typename Curve>
+__device__ __forceinline__ void design_fir_spectrum(SplitPlanes<double> planes, const cpx<double>* __restrict__ tw,
+                                                    const double* __restrict__ hann, Curve s, int ch, int parity, int ovs,
+                                                    double c0, double* __restrict__ fir_out, float2* __restrict__ H,
+                                                    mgb_track_state* state) {
+    const int tid = threadIdx.x, nthr = blockDim.x;
+    double* re = planes.re;
+    double* im = planes.im;
+    // ---- F: fir = ifftshift(irfft(s)) * hann (match_frequencies.py:98-99) ---------------------
+    // s is real, so its Hermitian extension X[k] = X[F-k] = s[k] is real and even and the inverse transform
+    // equals the forward one: all transforms of this kernel are ONE in-place forward FFT (design_fft, not
+    // inlined) -- the kernel runs once per CTA on cold instruction caches, and three unrolled copies of a
+    // float64 radix-16 FFT cost a third of its time in instruction fetches.
+    constexpr int PER = F / kDesignThreads;
+    static_assert(PER >= 1 && F % kDesignThreads == 0, "design: fft_size is a multiple of the block size");
+    double taps[PER];  // the thread's FIR taps tid + q*nthr
+    {
+#pragma unroll
+        for (int q = 0; q < PER; ++q) {
+            const int i = tid + q * kDesignThreads;
+            planes.store(i, cpx<double>{s(i <= F / 2 ? i : F - i), 0.0});
+        }
+        __syncthreads();
+        design_fft<F>(planes, tw);
+        __syncthreads();
+        const double inv = 1.0 / (double)F;
+#pragma unroll
+        for (int q = 0; q < PER; ++q) {
+            const int i = tid + q * kDesignThreads;
+            const int src = (i + F / 2) & (F - 1);
+            taps[q] = re[fft_pad(src)] * inv * hann[i];
+            if (fir_out && parity == 0) fir_out[(long long)ch * F + i] = taps[q];
+        }
+        __syncthreads();  // every tap has been read out of the planes
+    }
+
+    // ---- G: spectrum of the FIR on the ovs*F grid, bins 0..ovs*F/2 --------------------------------
+    // bin ovs*j + r = FFT_F(fir[n] * exp(-2*pi*i*r*n/(ovs*F)))[j].  ovs CTAs per channel: all have just designed
+    // the same FIR (steps A-F are cheap and deterministic), CTA r transforms it for the bins of residue r.
+    {
+        const double scale = c0 / ((double)ovs * (double)F);
+        float hpeak = 0.0f;  // max |H| of this CTA's bins: the convolution compares the two channels' peaks
+        const double step = -2.0 * (double)parity / ((double)ovs * (double)F);
+#pragma unroll
+        for (int q = 0; q < PER; ++q) {
+            const int i = tid + q * kDesignThreads;
+            double sn = 0.0, cs = 1.0;
+            if (parity != 0) sincospi(step * (double)i, &sn, &cs);
+            planes.store(i, cpx<double>{taps[q] * cs, taps[q] * sn});
+        }
+        __syncthreads();
+        design_fft<F>(planes, tw);
+        __syncthreads();
+        // bins ovs*j + parity <= ovs*F/2  (j = F/2 only for parity 0, where it wraps to the real bin F/2 of FFT_F)
+        const int jmax = (ovs * F / 2 - parity) / ovs;
+        for (int j = tid; j <= jmax; j += nthr) {
+            const int jj = j & (F - 1);
+            const float2 h = make_float2((float)(re[fft_pad(jj)] * scale), (float)(im[fft_pad(jj)] * scale));
+            H[ovs * j + parity] = h;
+            hpeak = fmaxf(hpeak, sqrtf(h.x * h.x + h.y * h.y));
+        }
+        __shared__ float red_peak[32];
+        hpeak = block_max(hpeak, red_peak);
+        if (tid == 0 && state) atomic_max_nonneg(ch == 0 ? &state->fir_peak_mid_bits : &state->fir_peak_side_bits, hpeak);
+    }
+}
+
 template <int F>
 __global__ void __launch_bounds__(kDesignThreads)
 design_kernel(mgb_plan plan, DesignArgs a) {
@@ -587,65 +658,51 @@ design_kernel(mgb_plan plan, DesignArgs a) {
     // ---- B-E: smoothing on the log-frequency grid, unless the operator kernel already produced s ---
     if (!a.s_ready) smooth_curve(plan, base);
 
-    // ---- F: fir = ifftshift(irfft(s)) * hann (match_frequencies.py:98-99) ---------------------
-    // s is real, so its Hermitian extension X[k] = X[F-k] = s[k] is real and even and the inverse transform
-    // equals the forward one: all transforms of this kernel are ONE in-place forward FFT (design_fft, not
-    // inlined) -- the kernel runs once per CTA on cold instruction caches, and three unrolled copies of a
-    // float64 radix-16 FFT cost a third of its time in instruction fetches.
-    constexpr int PER = F / kDesignThreads;
-    static_assert(PER >= 1 && F % kDesignThreads == 0, "design: fft_size is a multiple of the block size");
-    double taps[PER];  // the thread's FIR taps tid + q*nthr
-    {
-#pragma unroll
-        for (int q = 0; q < PER; ++q) {
-            const int i = tid + q * kDesignThreads;
-            planes.store(i, cpx<double>{s[i <= F / 2 ? i : F - i], 0.0});
-        }
-        __syncthreads();
-        design_fft<F>(planes, tw);
-        __syncthreads();
-        const double inv = 1.0 / (double)F;
-#pragma unroll
-        for (int q = 0; q < PER; ++q) {
-            const int i = tid + q * kDesignThreads;
-            const int src = (i + F / 2) & (F - 1);
-            taps[q] = re[fft_pad(src)] * inv * plan.d_hann[i];
-            if (a.fir_out && parity == 0) a.fir_out[(long long)ch * F + i] = taps[q];
-        }
-        __syncthreads();  // every tap has been read out of the planes
-    }
+    // ---- F-G: the FIR and its spectrum on the convolution's grid ----------------------------------
+    design_fir_spectrum<F>(planes, tw, plan.d_hann, [&](int k) { return s[k]; }, ch, parity, a.ovs, c0, a.fir_out,
+                           ch == 0 ? a.h_mid : a.h_side, a.state);
+}
 
-    // ---- G: spectrum of the FIR on the ovs*F grid, bins 0..ovs*F/2 --------------------------------
-    // bin ovs*j + r = FFT_F(fir[n] * exp(-2*pi*i*r*n/(ovs*F)))[j].  ovs CTAs per channel: all have just designed
-    // the same FIR (steps A-F are cheap and deterministic), CTA r transforms it for the bins of residue r.
-    {
-        float2* H = ch == 0 ? a.h_mid : a.h_side;
-        const int ovs = a.ovs;
-        const double scale = c0 / ((double)ovs * (double)F);
-        float hpeak = 0.0f;  // max |H| of this CTA's bins: the convolution compares the two channels' peaks
-        const double step = -2.0 * (double)parity / ((double)ovs * (double)F);
-#pragma unroll
-        for (int q = 0; q < PER; ++q) {
-            const int i = tid + q * kDesignThreads;
-            double sn = 0.0, cs = 1.0;
-            if (parity != 0) sincospi(step * (double)i, &sn, &cs);
-            planes.store(i, cpx<double>{taps[q] * cs, taps[q] * sn});
-        }
-        __syncthreads();
-        design_fft<F>(planes, tw);
-        __syncthreads();
-        // bins ovs*j + parity <= ovs*F/2  (j = F/2 only for parity 0, where it wraps to the real bin F/2 of FFT_F)
-        const int jmax = (ovs * F / 2 - parity) / ovs;
-        for (int j = tid; j <= jmax; j += nthr) {
-            const int jj = j & (F - 1);
-            const float2 h = make_float2((float)(re[fft_pad(jj)] * scale), (float)(im[fft_pad(jj)] * scale));
-            H[ovs * j + parity] = h;
-            hpeak = fmaxf(hpeak, sqrtf(h.x * h.x + h.y * h.y));
-        }
-        __shared__ float red_peak[32];
-        hpeak = block_max(hpeak, red_peak);
-        if (tid == 0 && a.state) atomic_max_nonneg(ch == 0 ? &a.state->fir_peak_mid_bits : &a.state->fir_peak_side_bits, hpeak);
-    }
+// ---- native-rate jobs: the analysis job's curve on the native rate's FIR grid --------------------------------
+// (mgb_match_frequencies_native; DESIGN.md section 4 "Native-rate masters")
+struct NativeDesignArgs {
+    const double* curve;        // the analysis job's smoothed curve of channel 0 (its parity-0 design block, at 2 n_lin)
+    long long curve_stride;     // doubles from channel 0's curve to channel 1's
+    const int* idx;             // [F/2 + 2] the native plan's tables (mgb_plan::d_native_idx, d_native_w)
+    const double* w;
+    double* scratch;            // the native workspace's design blocks (the float64 planes at F = 16384)
+    long long stride;
+    double* fir_out;            // [2][F] or null
+    float2* h_mid;
+    float2* h_side;
+    mgb_track_state* state;     // the native job's state: c0 from the analysis, the FIR peaks recorded here
+    int ovs;
+};
+
+// s'[j] = s[i] + w (s[i+1] - s[i]) up to the edge f_e; above it exp((1 - t) ln g_e), g_e = s(f_e) (the tables' last
+// entry), which crossfades to g_inf = 1 at R/2 and holds it; g_e <= 1 gives g_inf = g_e, a constant.  Then steps F-G
+// at the native length, exactly as design_kernel runs them.
+template <int F>
+__global__ void __launch_bounds__(kDesignThreads)
+design_native_kernel(mgb_plan plan, NativeDesignArgs a) {
+    constexpr int HB = F / 2 + 1;
+    MGB_DYN_SMEM(smem);
+    const int ch = blockIdx.x / a.ovs;
+    const int parity = blockIdx.x % a.ovs;
+    double* re = DesignSmem<F>::kGlobalPlanes
+                     ? a.scratch + ((long long)(kDesignBlocks * ch) + parity) * a.stride + (a.stride - 2 * DesignSmem<F>::kPlane)
+                     : reinterpret_cast<double*>(smem);
+    const SplitPlanes<double> planes{re, re + DesignSmem<F>::kPlane};
+    const double* s = a.curve + (long long)ch * a.curve_stride;
+    const double ge = s[a.idx[HB]] + a.w[HB] * (s[a.idx[HB] + 1] - s[a.idx[HB]]);
+    const double log_ge = ge > 1.0 ? log(ge) : 0.0;
+    auto curve = [&](int j) {
+        const int i = a.idx[j];
+        if (i >= 0) return s[i] + a.w[j] * (s[i + 1] - s[i]);
+        return ge > 1.0 ? exp((1.0 - a.w[j]) * log_ge) : ge;
+    };
+    design_fir_spectrum<F>(planes, (const cpx<double>*)plan.d_tw_f64_F, plan.d_hann, curve, ch, parity, a.ovs,
+                           a.state->rms_coefficient, a.fir_out, ch == 0 ? a.h_mid : a.h_side, a.state);
 }
 
 __global__ void ratio_kernel(const double* __restrict__ avg, double* __restrict__ scratch, long long stride, int n_lin,
@@ -866,6 +923,38 @@ int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Wo
         default: break;
     }
     set_error("design: fft_size %d has no kernel", plan.fft_size);
+    return MGB_ERR_UNSUPPORTED;
+}
+
+int launch_design_native(const mgb_plan& plan, const Workspace& ws, const mgb_plan& nplan, const mgb_track_layout& nlayout,
+                         const Workspace& nws, double* fir_out, mgb_track_state* nstate, cudaStream_t stream) {
+    NativeDesignArgs a;
+    a.curve = ws.design + 2LL * plan.n_lin;
+    a.curve_stride = (long long)kDesignBlocks * ws.design_stride;
+    a.idx = nplan.d_native_idx;
+    a.w = nplan.d_native_w;
+    a.scratch = nws.design;
+    a.stride = nws.design_stride;
+    a.fir_out = fir_out;
+    a.h_mid = nws.h_mid;
+    a.h_side = nws.h_side;
+    a.state = nstate;
+    a.ovs = conv_frame_ovs(nplan.fft_size, nlayout.target_piece);
+#define MGB_NATIVE_CASE(FF)                                                                                           \
+    case FF:                                                                                                          \
+        return launch("design_native_kernel<" #FF ">", design_native_kernel<FF>, dim3(2 * a.ovs), dim3(kDesignThreads), \
+                      DesignSmem<FF>::kBytes, stream, nplan, a);
+    switch (nplan.fft_size) {
+        MGB_NATIVE_CASE(512)
+        MGB_NATIVE_CASE(1024)
+        MGB_NATIVE_CASE(2048)
+        MGB_NATIVE_CASE(4096)
+        MGB_NATIVE_CASE(8192)
+        MGB_NATIVE_CASE(16384)
+        default: break;
+    }
+#undef MGB_NATIVE_CASE
+    set_error("design_native: fft_size %d has no kernel", nplan.fft_size);
     return MGB_ERR_UNSUPPORTED;
 }
 

@@ -123,6 +123,9 @@ int launch_analyze(const mgb_plan& plan, const float2* x, int64_t frames, int64_
 int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Workspace& ws,
                   const double* avg_override, double* fir_out, mgb_track_state* state, cudaStream_t stream);
 int64_t design_doubles_per_channel(const mgb_plan& plan);
+// native-rate jobs: the curve launch_design left in `ws` (plan's job) -> the FIR of nplan's length and its spectra in `nws`
+int launch_design_native(const mgb_plan& plan, const Workspace& ws, const mgb_plan& nplan, const mgb_track_layout& nlayout,
+                         const Workspace& nws, double* fir_out, mgb_track_state* nstate, cudaStream_t stream);
 // the reference's analysis partials (ReferenceRegions) -> a profile blob at `out` (header + spectra)
 int launch_reference_profile(const mgb_plan& plan, const ReferenceGeometry& g, const ReferenceRegions& r,
                              mgb_reference_profile* out, cudaStream_t stream);

@@ -42,7 +42,8 @@ class Config:
                  lowess_frac: float = 0.0375, lowess_it: int = 0, lowess_delta: float = 0.001,
                  preview_size: float = 30, preview_analysis_step: float = 5, preview_fade_size: float = 1,
                  preview_fade_coefficient: float = 8, temp_folder: str = None,
-                 limiter: LimiterConfig = None, true_peak: bool = False, loudness_target: float = None):
+                 limiter: LimiterConfig = None, true_peak: bool = False, loudness_target: float = None,
+                 native_rate: bool = False):
         sr = internal_sample_rate
         _require(isinstance(sr, int) and sr > 0, "internal_sample_rate must be a positive int")
         if sr != 44100:
@@ -74,6 +75,7 @@ class Config:
             limiter = _DEFAULT_LIMITER
         _require(isinstance(limiter, LimiterConfig), "limiter must be a LimiterConfig")
         _require(isinstance(true_peak, bool), "true_peak must be a bool")
+        _require(isinstance(native_rate, bool), "native_rate must be a bool")
         _require(loudness_target is None or (isinstance(loudness_target, (int, float)) and not isinstance(loudness_target, bool)
                                              and math.isfinite(loudness_target) and -70 < loudness_target < 0),
                  "loudness_target must be None or a finite LUFS value in (-70, 0)")
@@ -104,6 +106,10 @@ class Config:
         # LUFS: the limited outputs are driven into the limiter until they read this integrated loudness (a search on
         # the device; final_amplitude_coefficient is not applied there).  None: the reference's level, as before
         self.loudness_target = None if loudness_target is None else float(loudness_target)
+        # True: mg.process masters a target whose file rate differs from internal_sample_rate at that rate.  The match
+        # is still analysed on a copy resampled to internal_sample_rate; the FIR, the corrections, the limiter and every
+        # result then run on the target's own samples.  False: the reference's behaviour, every result at the internal rate
+        self.native_rate = native_rate
 
 
 _DEFAULT_LIMITER = LimiterConfig()  # shared default instance, like the reference's default argument

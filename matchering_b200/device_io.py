@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from . import _native, wavio
-from .checker import peak_warning
+from .checker import peak_warning, resampled_for_analysis
 from .defaults import Config
 from .engine import _require_cuda, _stream_ptr
 from .log import Code, ModuleError, debug, info, warning
@@ -46,10 +46,11 @@ def load_to_device(file: str, file_type: str, config: Config):
     return out, rate
 
 
-def check_on_device(audio: torch.Tensor, config: Config, name: str, sample_rate: int = None) -> torch.Tensor:
+def check_on_device(audio: torch.Tensor, config: Config, name: str, sample_rate: int = None, native: bool = False):
     """matchering/checker.py:90-137 for a signal that is already on the device, in the reference's order: length
     limits at the SOURCE rate, mono -> stereo, resampling to the internal rate (csrc/resample.cu), and (target
-    only) the clipping / limiter detection."""
+    only) the clipping / limiter detection.  native (the target of a Config(native_rate=True) job): -> (audio, the
+    stereo signal at its own rate), as checker.check."""
     name = name.upper()
     is_target = name == "TARGET"
     frames, channels = audio.shape
@@ -65,12 +66,16 @@ def check_on_device(audio: torch.Tensor, config: Config, name: str, sample_rate:
     if channels == 1:
         info(Code.INFO_TARGET_IS_MONO if is_target else Code.INFO_REFERENCE_IS_MONO)
         audio = audio.repeat(1, 2).contiguous()
+    source = audio
     if sample_rate != sr:
         from .resample import resample_on_device
         debug(f"Resampling {name} audio from {sample_rate} Hz to {sr} Hz...")
         audio = resample_on_device(audio, sample_rate, sr)
         frames = audio.shape[0]
-        (warning if is_target else info)(Code.WARNING_TARGET_IS_RESAMPLED if is_target else Code.INFO_REFERENCE_IS_RESAMPLED)
+        if native:
+            debug(resampled_for_analysis(sample_rate, config))
+        else:
+            (warning if is_target else info)(Code.WARNING_TARGET_IS_RESAMPLED if is_target else Code.INFO_REFERENCE_IS_RESAMPLED)
     if is_target:
         lib = _native.load()
         scratch = torch.zeros(16, dtype=torch.uint8, device=audio.device)
@@ -81,7 +86,7 @@ def check_on_device(audio: torch.Tensor, config: Config, name: str, sample_rate:
         code = peak_warning(peak, hits, config)  # matchering/checker.py:75-87
         if code is not None:
             warning(code)
-    return audio
+    return (audio, source) if native else audio
 
 
 def check_equality_on_device(target: torch.Tensor, reference: torch.Tensor) -> None:

@@ -28,11 +28,16 @@ def _stream_ptr(device) -> C.c_void_p:
 
 
 class DevicePlan:
-    def __init__(self, config, device: torch.device):
+    """`native_tables` (plan.native_tables): the plan of a native-rate job's stages 2-4, which designs no curve of its
+    own -- it carries the analysis plan's over -- and so builds no smoothing operator."""
+
+    def __init__(self, config, device: torch.device, native_tables: dict | None = None):
         self.lib = _native.load()
         self.device = device
         self.tables = _plan.build_tables(config)
         t = self.tables
+        if native_tables is not None:
+            t.arrays.update(native_tables)
         s = _native.Plan()
         s.sample_rate, s.fft_size, s.n_lin, s.n_log = t.sample_rate, t.fft_size, t.n_lin, t.n_log
         s.rms_correction_steps, s.lowess_k = t.rms_correction_steps, t.lowess_k
@@ -55,7 +60,7 @@ class DevicePlan:
         self.struct = s
         with torch.cuda.device(device):
             _native.check(self.lib, self.lib.mgb_plan_fill_twiddles(C.byref(s), _stream_ptr(device)))
-            if t.lowess_it > 0 or t.fft_size > _plan.OPERATOR_MAX_FFT_SIZE:
+            if t.lowess_it > 0 or t.fft_size > _plan.OPERATOR_MAX_FFT_SIZE or native_tables is not None:
                 return  # robustness iterations make the smoothing non-linear in the data: direct chain per track
             # the smoothing chain as one Config-only matrix, built on the device from the direct kernels
             ws_bytes = int(self.lib.mgb_plan_operator_workspace_bytes(C.byref(s)))
@@ -96,6 +101,18 @@ def get_plan(config, device=None) -> DevicePlan:
     plan = _PLAN_CACHE.get(key)
     if plan is None:
         plan = _PLAN_CACHE[key] = DevicePlan(config, device)
+    return plan
+
+
+def get_native_plan(config, rate: int, device=None) -> DevicePlan:
+    """The plan of stages 2-4 of a native-rate job at `rate` (plan.native_config), with the tables that carry the
+    analysis curve of `config`'s plan over to its FIR; cached per device, Config and rate."""
+    _require_cuda()
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    key = (device.index, _plan.config_key(config), "native", int(rate))
+    plan = _PLAN_CACHE.get(key)
+    if plan is None:
+        plan = _PLAN_CACHE[key] = DevicePlan(_plan.native_config(config, rate), device, _plan.native_tables(config, rate))
     return plan
 
 
@@ -168,6 +185,25 @@ class TrackSession:
         _native.check(self.lib, self.lib.mgb_match_frequencies(
             p, l, target.data_ptr(), self.result.data_ptr(), fir_out.data_ptr() if fir_out is not None else None,
             self.workspace.data_ptr(), self.state.data_ptr(), _stream_ptr(self.device)))
+
+    def design_frequencies(self, fir_out: torch.Tensor | None = None) -> None:
+        """Stage 2's FIR design without its convolution (mgb_design_frequencies): what a native-rate job takes from
+        its analysis session."""
+        p, l = self._args()
+        _native.check(self.lib, self.lib.mgb_design_frequencies(
+            p, l, fir_out.data_ptr() if fir_out is not None else None, self.workspace.data_ptr(), self.state.data_ptr(),
+            _stream_ptr(self.device)))
+
+    def match_frequencies_native(self, analysis: "TrackSession", target: torch.Tensor,
+                                 fir_out: torch.Tensor | None = None) -> None:
+        """Stage 2 of a native-rate job in this session (a native plan's, profiled layout): the FIR carried over from
+        `analysis`, which has run match_levels and design_frequencies, then the convolution of `target` at this rate."""
+        p, l = analysis._args()
+        np_, nl = self._args()
+        _native.check(self.lib, self.lib.mgb_match_frequencies_native(
+            p, l, analysis.workspace.data_ptr(), analysis.state.data_ptr(), np_, nl, target.data_ptr(),
+            self.result.data_ptr(), fir_out.data_ptr() if fir_out is not None else None, self.workspace.data_ptr(),
+            self.state.data_ptr(), _stream_ptr(self.device)))
 
     def correct_levels(self) -> None:
         p, l = self._args()

@@ -25,6 +25,7 @@ from scipy import signal as _signal
 
 SUPPORTED_FFT_SIZES = (512, 1024, 2048, 4096, 8192, 16384)
 OPERATOR_MAX_FFT_SIZE = 8192  # above: no Config-only smoothing matrix (its row bands would be 80 MB), direct chain per track
+NATIVE_EDGE = 0.9  # native-rate jobs: the analysis curve is trusted up to 0.9 * R/2, below the resampler's roll-off
 
 
 class UnsupportedConfig(NotImplementedError):
@@ -345,3 +346,59 @@ def build_tables(config) -> PlanTables:
         arrays[name] = np.ascontiguousarray(arr, dtype=want)
     return PlanTables(sr, F, n_lin, n_log, config.rms_correction_steps, k, int(config.lowess_it), float(config.max_piece_size),
                       config.threshold, config.min_value, limiter_constants(config), arrays)
+
+
+# ------------------------------------------------------------------------------------------------
+# native-rate jobs (Config(native_rate=True); DESIGN.md section 4 "Native-rate masters")
+# ------------------------------------------------------------------------------------------------
+def native_fft_size(config, rate: int) -> int:
+    """F' = F * 2^round(log2(R'/R)): the native FIR keeps the analysis FIR's length in seconds to within a factor of
+    sqrt(2), and so its frequency resolution.  UnsupportedConfig where no kernel exists for it."""
+    R, F = config.internal_sample_rate, config.fft_size
+    size = F * 2.0 ** math.floor(math.log2(rate / R) + 0.5)
+    if size not in SUPPORTED_FFT_SIZES:
+        raise UnsupportedConfig(f"a {rate} Hz target at internal_sample_rate={R}, fft_size={F} needs a native FIR of "
+                                f"{size:.0f} points: kernels exist for {SUPPORTED_FFT_SIZES}")
+    return int(size)
+
+
+def native_config(config, rate: int):
+    """The Config stages 2-4 of a native-rate job run under: `config` at `rate`, every seconds-valued field the same
+    length in seconds, fft_size = native_fft_size."""
+    import copy
+    R = config.internal_sample_rate
+    out = copy.copy(config)
+    out.fft_size = native_fft_size(config, rate)
+    out.internal_sample_rate = int(rate)
+    for name in ("max_piece_size", "preview_size", "preview_analysis_step", "preview_fade_size"):
+        setattr(out, name, getattr(config, name) / R * rate)
+    return out
+
+
+def native_check_length(config, rate: int, frames: int) -> None:
+    """A native target must give the native FIR what the analysis FIR needs at R: more frames than F' and pieces
+    (match_levels.py:47-59 at R') of at least F' frames.  ValueError otherwise, before anything runs."""
+    nc = native_config(config, rate)
+    F = nc.fft_size
+    piece = int(frames / (int(frames / nc.max_piece_size) + 1))
+    if frames <= F or piece < F:
+        raise ValueError(f"a target of {frames} frames at {rate} Hz is too short for the native FIR of {F} points "
+                         f"(pieces of {piece} frames)")
+
+
+def native_tables(config, rate: int) -> dict:
+    """mgb_plan::d_native_idx / d_native_w of the native plan at `rate`: for j = 0 .. F'/2 at f_j = j R'/F', the
+    analysis curve's bin i and weight w of s'[j] = s[i] + w (s[i+1] - s[i]) at position f_j F/R while f_j <= f_e, and
+    above f_e (idx -1) the crossfade position t = (f_j - f_e) / (R/2 - f_e), held at 1 from R/2 on.  Entry F'/2 + 1
+    is the edge f_e itself."""
+    R, F = config.internal_sample_rate, config.fft_size
+    Fn = native_fft_size(config, rate)
+    hb = Fn // 2 + 1
+    f_e = NATIVE_EDGE * R / 2
+    f = np.append(np.arange(hb) * (rate / Fn), f_e)
+    inside = f <= f_e
+    pos = f * (F / R)
+    i = np.minimum(np.floor(pos), F // 2 - 1)
+    idx = np.where(inside, i, -1).astype(np.int32)
+    w = np.where(inside, pos - i, np.minimum((f - f_e) / (R / 2 - f_e), 1.0))
+    return {"native_idx": np.ascontiguousarray(idx), "native_w": np.ascontiguousarray(w, dtype=np.float64)}

@@ -5,10 +5,10 @@ from __future__ import annotations
 
 import torch
 
-from . import _native
+from . import _native, plan as _plan
 from .defaults import Config
-from .engine import (TrackSession, get_plan, host_array_ok, stages_main_host, stages_main_host_profiled, to_device_f32,
-                     to_host_like)
+from .engine import (TrackSession, get_native_plan, get_plan, host_array_ok, stages_main_host, stages_main_host_profiled,
+                     to_device_f32, to_host_like)
 from .log import Code, info, debug, debug_line, debug_enabled
 from .profile import ReferenceProfile
 from .utils import to_db
@@ -121,6 +121,93 @@ def main_device(target, reference, config: Config, need_default: bool = True, ne
 
         if debug_enabled():  # one read-back of the device scalars, only when somebody listens
             _debug_scalars(session.read_state(), session.layout, reference if profiled else None)
+            if report is not None:
+                from .loudness import LoudnessTarget, debug_target
+                raw = report.cpu().numpy().tobytes()
+                debug_target(LoudnessTarget.from_report(config.loudness_target,
+                                                        _native.LoudnessTargetReport.from_buffer_copy(raw)))
+
+    return limited, plain, normalized
+
+
+def main_native(target, sample_rate: int, reference, config: Config, need_default: bool = True,
+                need_no_limiter: bool = False, need_no_limiter_normalized: bool = False):
+    """`main` for a target at its own rate `sample_rate` (DESIGN.md section 4 "Native-rate masters"): the level and
+    spectrum match is analysed on the target resampled to config.internal_sample_rate, as `main` would see it, and the
+    FIR, the RMS correction, the limiter (true peak, loudness target) then run on the target's own samples, so every
+    output is at `sample_rate` with the target's length.  target: (N, 2) or mono (N, 1), numpy or torch; the outputs
+    come back in its array type.  At sample_rate == internal_sample_rate this is `main`."""
+    if int(sample_rate) == config.internal_sample_rate:
+        return main(target, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
+    outs = main_native_device(target, sample_rate, reference, config, need_default, need_no_limiter,
+                              need_no_limiter_normalized)
+    return tuple(None if t is None else to_host_like(t, target) for t in outs)
+
+
+def main_native_device(target, sample_rate: int, reference, config: Config, need_default: bool = True,
+                       need_no_limiter: bool = False, need_no_limiter_normalized: bool = False, analysis=None):
+    """`main_native` with the results left on the device as float32 CUDA tensors.  `analysis`: the target already
+    resampled to the internal rate (mg.process's loaders make it while checking the target); made here otherwise."""
+    sample_rate = int(sample_rate)
+    if sample_rate == config.internal_sample_rate:
+        return main_device(target, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
+    profiled = isinstance(reference, ReferenceProfile)
+    if profiled:
+        reference.check_config(config)
+    if target.ndim != 2 or target.shape[1] not in (1, 2) or (not profiled and (reference.ndim != 2 or reference.shape[1] != 2)):
+        raise ValueError("the target must be (frames, 2) or (frames, 1) and the reference (frames, 2)")
+    _plan.native_check_length(config, sample_rate, int(target.shape[0]))  # (raises before any device work)
+    plan = get_plan(config)
+    nplan = get_native_plan(config, sample_rate, plan.device)
+    device = plan.device
+    with torch.cuda.device(device):
+        d_native = to_device_f32(target, device)
+        if d_native.shape[1] == 1:
+            d_native = d_native.repeat(1, 2).contiguous()
+        if analysis is None:
+            from .resample import resample_on_device
+            d_target = resample_on_device(d_native, sample_rate, config.internal_sample_rate)
+        else:
+            d_target = to_device_f32(analysis, device)
+        if profiled:
+            d_profile = reference.checked_blob(plan)
+            session = TrackSession(plan, d_target.shape[0], None)
+        else:
+            d_reference = to_device_f32(reference, device)
+            session = TrackSession(plan, d_target.shape[0], d_reference.shape[0])
+        native = TrackSession(nplan, d_native.shape[0], None)
+
+        debug_line()
+        info(Code.INFO_MATCHING_LEVELS)          # stages.py:52
+        debug(f"The maximum size of the analyzed piece: {config.max_piece_size} samples "
+              f"or {config.max_piece_size / config.internal_sample_rate:.2f} seconds")
+        if profiled:
+            session.match_levels_profiled(d_target, d_profile)
+        else:
+            session.match_levels(d_target, d_reference)
+
+        debug_line()
+        info(Code.INFO_MATCHING_FREQS)           # stages.py:117
+        debug(f"The FIR is designed at {config.internal_sample_rate} Hz and applied at {sample_rate} Hz "
+              f"({nplan.tables.fft_size} points)")
+        session.design_frequencies()
+        native.match_frequencies_native(session, d_native)
+
+        debug_line()
+        info(Code.INFO_CORRECTING_LEVELS)        # stages.py:147
+        native.correct_levels()
+
+        debug_line()
+        info(Code.INFO_FINALIZING)               # stages.py:182
+        report = None
+        if need_default and config.loudness_target is not None:
+            limited, plain, normalized, report = native.finalize_to_loudness(config.loudness_target, need_no_limiter,
+                                                                             need_no_limiter_normalized)
+        else:
+            limited, plain, normalized = native.finalize(need_default, need_no_limiter, need_no_limiter_normalized)
+
+        if debug_enabled():
+            _debug_scalars(native.read_state(), session.layout, reference if profiled else None)
             if report is not None:
                 from .loudness import LoudnessTarget, debug_target
                 raw = report.cpu().numpy().tobytes()
