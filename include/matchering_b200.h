@@ -302,6 +302,37 @@ int mgb_match_frequencies_native(const mgb_plan* plan, const mgb_track_layout* l
                                  const mgb_track_layout* native_layout, const float* d_native_target, float* d_native_result,
                                  double* d_fir_out, void* d_native_workspace, mgb_track_state* d_native_state, void* stream);
 
+/* ---- album mastering: one level match and one matching FIR for K tracks (DESIGN.md section 4) --------------------
+ * Stages 1-3 of K jobs whose reference comes from one profile, with their statistics pooled over the album:
+ *   - stage 1: every piece (t, p) of every track counts once in the average, the loud mask and the match RMS
+ *     (match_levels.py:62-71 over the union of the tracks' pieces); one c0 = reference match RMS / max(eps, album match);
+ *   - stage 2: the target spectra are the mean |rfft| over every boxcar frame of every loud piece of every track, ONE
+ *     FIR is designed from them and every track is convolved with it (each track picks its float32 or float64
+ *     convolution from its own peak, as a single job does);
+ *   - stage 3: each step's coefficient comes from the per-piece sums of all tracks, pooled the same way, and multiplies
+ *     every track.
+ * Each track keeps its own piece layout.  After the call every track is where mgb_correct_levels leaves a single job:
+ * the caller runs mgb_finalize (or mgb_finalize_to_loudness) per track with its layout, workspace and state.  A one-track
+ * album computes bit for bit what the profiled job computes.  The tracks' analysis, convolution and finalize kernels are
+ * the single job's; the pooled steps are one launch each over all tracks. */
+#define MGB_MAX_ALBUM_TRACKS 64
+typedef struct mgb_album_track {
+    const mgb_track_layout* layout; /* mgb_track_layout_init_profiled of the plan */
+    const float* d_target_lr;       /* layout->target_frames stereo frames at the plan's rate */
+    float* d_result_lr;             /* the stage-2 result, as mgb_match_frequencies writes it (not d_target_lr) */
+    void* d_workspace;              /* layout->workspace_bytes */
+    mgb_track_state* d_state;
+} mgb_album_track;
+/* device scratch of the album's design (the FIR's spectra on both convolution grids); -1 for bad arguments */
+int64_t mgb_album_workspace_bytes(const mgb_plan* plan, int32_t tracks, const mgb_track_layout* layouts);
+/* MGB_ERR_INVALID: no tracks or more than MGB_MAX_ALBUM_TRACKS, NULL or misaligned pointers, a layout that is not a
+ * profiled layout of this plan, a result buffer that is its track's target, a profile whose header does not match the
+ * plan (mgb_reference_profile_check; the call reads the header back, which waits for `stream`).  MGB_ERR_WORKSPACE: a
+ * short album workspace.  MGB_ERR_UNSUPPORTED: more pieces than the pooled statistics fit in one CTA's shared memory.
+ * d_fir_out (optional): [2][F] doubles, the album's mid and side FIRs. */
+int mgb_album_match(const mgb_plan* plan, int32_t tracks, const mgb_album_track* t, const void* d_profile, double* d_fir_out,
+                    void* d_album_ws, int64_t album_ws_bytes, void* stream);
+
 /* ---- stage 3: stages.__correct_levels (stages.py:138-170) -----------------------------------
  * rms_correction_steps iterations of clip -> per-piece RMS -> loudest mask -> coefficient.  The
  * coefficients accumulate in d_state->gain; the samples are scaled once, by the consumer.  A step

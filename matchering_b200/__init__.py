@@ -19,3 +19,8 @@ from .loudness import Loudness, loudness  # (the function shadows the module nam
 def process(*args, **kwargs):
     from .core import process as _process
     return _process(*args, **kwargs)
+
+
+def process_album(*args, **kwargs):
+    from .core import process_album as _process_album
+    return _process_album(*args, **kwargs)

@@ -133,6 +133,17 @@ class TrackLayout(C.Structure):
     ]
 
 
+class AlbumTrack(C.Structure):
+    """mgb_album_track: one track of mgb_album_match (device pointers)."""
+    _fields_ = [
+        ("layout", C.POINTER(TrackLayout)), ("d_target_lr", C.c_void_p), ("d_result_lr", C.c_void_p),
+        ("d_workspace", C.c_void_p), ("d_state", C.c_void_p),
+    ]
+
+
+MGB_MAX_ALBUM_TRACKS = 64
+
+
 MGB_REFERENCE_PROFILE_VERSION = 1
 
 
@@ -236,6 +247,9 @@ PROTOTYPES = {
     "mgb_match_frequencies_native": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p,
                                                C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mgb_album_workspace_bytes": (C.c_int64, [C.POINTER(Plan), C.c_int32, C.POINTER(TrackLayout)]),
+    "mgb_album_match": (C.c_int, [C.POINTER(Plan), C.c_int32, C.POINTER(AlbumTrack), C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_int64, C.c_void_p]),
     "mgb_correct_levels": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_finalize": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -79,6 +79,82 @@ def process(target: str, reference, results: list, config: Config = None,
     info(Code.INFO_COMPLETED)
 
 
+def process_album(targets: list, reference, results: list, config: Config = None):
+    """Master an album: `targets` is a list of file paths, `results` a list of the same length whose entries are lists
+    of Result as mg.process takes them.  Every target is loaded and checked as mg.process loads its target; then ONE
+    level match and ONE matching FIR, from statistics pooled over every track (stages.main_album), master them all, so
+    the tracks keep their relative levels.  `reference` is a file path or a ReferenceProfile.  Config(loudness_target=...)
+    and native-rate targets are refused."""
+    from .stages import album_check, main_album_device
+    if config is None:
+        config = Config()
+    targets, results = list(targets), list(results)
+    if not targets or len(targets) != len(results):
+        raise ValueError(f"process_album: {len(targets)} targets and {len(results)} result lists")
+    album_check(len(targets), config)
+    if any(not r for r in results):
+        raise ValueError("process_album: every track needs at least one Result")
+    if config.native_rate:
+        for t in targets:
+            rate = _file_rate(t)
+            if rate is not None and rate != config.internal_sample_rate:
+                raise ValueError(f"process_album: '{t}' is at {rate} Hz; albums are mastered at the internal rate "
+                                 f"({config.internal_sample_rate} Hz), not at native rates")
+    debug_line()
+    info(Code.INFO_LOADING)
+    temp_folder = config.temp_folder if config.temp_folder else get_temp_folder([r for rs in results for r in rs])
+    reference_audio = None
+    if isinstance(reference, ReferenceProfile):
+        reference.check_config(config)
+    else:
+        reference_audio, reference_rate = _load_and_check(reference, "reference", temp_folder, config)
+        if (reference_rate != config.internal_sample_rate or reference_audio.shape[1] != 2
+                or not reference_audio.shape[0] > config.fft_size):
+            raise ModuleError(Code.ERROR_VALIDATION)
+    audios = []
+    for t in targets:
+        audio, rate, _, native_rate = _load_and_check_target(t, temp_folder, config)
+        if native_rate != config.internal_sample_rate:
+            raise ValueError(f"process_album: '{t}' is at {native_rate} Hz; albums are mastered at the internal rate")
+        if reference_audio is not None and not config.allow_equality:
+            _check_equality_any(audio, reference_audio)
+        if rate != config.internal_sample_rate or audio.shape[1] != 2 or not audio.shape[0] > config.fft_size:
+            raise ModuleError(Code.ERROR_VALIDATION)
+        audios.append(audio)
+    if reference_audio is not None:
+        from .profile import analyze_reference
+        reference = analyze_reference(reference_audio, config)
+
+    everything = [r for rs in results for r in rs]
+    needs = dict(need_default=any(r.use_limiter for r in everything),
+                 need_no_limiter=any(not r.use_limiter and not r.normalize for r in everything),
+                 need_no_limiter_normalized=any(not r.use_limiter and r.normalize for r in everything))
+    outs = main_album_device(audios, reference, config, **needs)
+    debug_line()
+    info(Code.INFO_EXPORTING)
+    for (limited, plain, normalized), wanted_list in zip(outs, results):
+        for wanted in wanted_list:
+            audio = limited if wanted.use_limiter else (normalized if wanted.normalize else plain)
+            _export(wanted, audio, config.internal_sample_rate)
+    debug_line()
+    info(Code.INFO_COMPLETED)
+
+
+def _file_rate(path) -> int | None:
+    """The sample rate a file's header states, or None when it cannot be read without decoding."""
+    from . import wavio
+    from .results import real_soundfile
+    try:
+        with open(path, "rb") as f:
+            layout = wavio._pcm_layout(f)
+        if layout is not None:
+            return layout[2]
+        sf = real_soundfile()
+        return int(sf.info(path).samplerate) if sf is not None else None
+    except (OSError, RuntimeError):
+        return None
+
+
 def _export(wanted: Result, audio, sample_rate: int, name: str = "result") -> None:
     """16/24-bit WAV results are quantised on the device and written as they come back (a quarter of
     the device->host bytes of a float64 array); everything else takes the reference's route through

@@ -713,6 +713,138 @@ int mgb_match_frequencies_native(const mgb_plan* plan, const mgb_track_layout* L
                            d_native_state, st);
 }
 
+// ---- album mastering ----------------------------------------------------------------------------------------------
+// The album workspace: the design blocks of one job, then the FIR's spectra (mid, side) on the 2F-point and on the
+// 4F-point grid (a track's convolution grid follows from its piece length, conv_frame_ovs).
+struct AlbumRegions {
+    double* design;
+    int64_t design_stride;
+    float2* h[2][2];  // [grid: 2F, 4F][mid, side]
+    int64_t total_bytes;
+};
+static AlbumRegions carve_album(const mgb_plan& plan, void* base_ptr) {
+    AlbumRegions r;
+    const uintptr_t base = reinterpret_cast<uintptr_t>(base_ptr);
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) {
+        unsigned char* p = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
+        off += align256(bytes);
+        return p;
+    };
+    r.design_stride = (design_doubles_per_channel(plan) + 31) / 32 * 32;
+    r.design = (double*)take(8 * r.design_stride * 8);
+    for (int g = 0; g < 2; ++g)
+        for (int c = 0; c < 2; ++c) r.h[g][c] = (float2*)take((2LL * plan.fft_size + 1) * 8);
+    r.total_bytes = off;
+    return r;
+}
+
+// a profiled layout of this plan for its own target length, as mgb_track_layout_init_profiled makes it
+static int check_album_layout(const mgb_plan* plan, const mgb_track_layout* L, int t) {
+    MGB_REQUIRE(L != nullptr, MGB_ERR_INVALID, "album: track %d has no layout", t);
+    MGB_REQUIRE(layout_profiled(*L) && L->target_frames > plan->fft_size, MGB_ERR_INVALID,
+                "album: track %d: the layout is not a profiled layout of this plan, or the track is not longer than fft_size", t);
+    mgb_track_layout want;
+    if (mgb_track_layout_init_profiled(plan, L->target_frames, &want) != MGB_OK ||
+        memcmp(&want, L, sizeof(want)) != 0) {
+        set_error("album: track %d: the layout is not this plan's profiled layout of %lld frames", t, (long long)L->target_frames);
+        return MGB_ERR_INVALID;
+    }
+    return MGB_OK;
+}
+
+int64_t mgb_album_workspace_bytes(const mgb_plan* plan, int32_t tracks, const mgb_track_layout* layouts) {
+    if (check_plan(plan) != MGB_OK || tracks < 1 || tracks > MGB_MAX_ALBUM_TRACKS || layouts == nullptr) return -1;
+    for (int t = 0; t < tracks; ++t)
+        if (check_album_layout(plan, &layouts[t], t) != MGB_OK) return -1;
+    return carve_album(*plan, nullptr).total_bytes;
+}
+
+int mgb_album_match(const mgb_plan* plan, int32_t tracks, const mgb_album_track* t, const void* d_profile, double* d_fir_out,
+                    void* d_album_ws, int64_t album_ws_bytes, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(tracks >= 1 && tracks <= MGB_MAX_ALBUM_TRACKS, MGB_ERR_INVALID, "album: %d tracks (1 .. %d)", (int)tracks,
+                MGB_MAX_ALBUM_TRACKS);
+    MGB_REQUIRE(t != nullptr, MGB_ERR_INVALID, "album: the track table is NULL");
+    std::vector<AlbumTrack> album((size_t)tracks);
+    for (int k = 0; k < tracks; ++k) {
+        MGB_TRY(check_album_layout(plan, t[k].layout, k));
+        MGB_TRY(check_aligned(t[k].d_target_lr, "d_target_lr"));
+        MGB_TRY(check_aligned(t[k].d_result_lr, "d_result_lr"));
+        MGB_TRY(check_aligned(t[k].d_workspace, "d_workspace"));
+        MGB_TRY(check_aligned(t[k].d_state, "d_state"));
+        MGB_REQUIRE((const void*)t[k].d_result_lr != (const void*)t[k].d_target_lr, MGB_ERR_INVALID,
+                    "album: track %d: d_result_lr is its d_target_lr", k);
+        // (the analysis partials are addressed as 16-bit item numbers in the pooled kernel)
+        MGB_REQUIRE((int64_t)t[k].layout->target_divisions * t[k].layout->target_slots < 65536, MGB_ERR_UNSUPPORTED,
+                    "album: track %d has too many analysis items", k);
+        album[k].layout = *t[k].layout;
+        album[k].ws = carve_workspace(*plan, *t[k].layout, t[k].d_workspace);
+        album[k].state = t[k].d_state;
+    }
+    MGB_TRY(check_aligned(d_profile, "d_profile"));
+    MGB_TRY(check_aligned(d_album_ws, "d_album_ws"));
+    const AlbumRegions need = carve_album(*plan, nullptr);
+    MGB_REQUIRE(album_ws_bytes >= need.total_bytes, MGB_ERR_WORKSPACE, "album: workspace of %lld bytes, need %lld",
+                (long long)album_ws_bytes, (long long)need.total_bytes);
+    MGB_REQUIRE(album_mean_smem(album.data(), tracks) <= 227 * 1024, MGB_ERR_UNSUPPORTED,
+                "album: %zu bytes of pooled piece statistics exceed one CTA's shared memory", album_mean_smem(album.data(), tracks));
+    cudaStream_t st = (cudaStream_t)stream;
+    {
+        mgb_reference_profile h;
+#ifdef MGB_EMULATE
+        memcpy(&h, d_profile, sizeof(h));
+#else
+        if (cudaMemcpyAsync(&h, d_profile, sizeof(h), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            cudaStreamSynchronize(st) != cudaSuccess)
+            return cuda_status("album: profile header");
+#endif
+        MGB_TRY(mgb_reference_profile_check(plan, &h));
+    }
+    // stage 1: each track's analysis, as its profiled job runs it
+    for (int k = 0; k < tracks; ++k)
+        MGB_TRY(mgb_match_levels_profiled(plan, t[k].layout, t[k].d_target_lr, d_profile, t[k].d_workspace, t[k].d_state,
+                                          stream));
+    // the album's level statistics and matching curve, then one FIR per convolution grid the tracks use; the first
+    // track on a grid receives the FIR's peaks, the others copy them
+    const AlbumRegions r = carve_album(*plan, d_album_ws);
+    MGB_TRY(launch_album_mean(*plan, album.data(), tracks, album[0].ws.profile, r.design, r.design_stride, st));
+    int leader[2] = {-1, -1};
+    double* fir_out = d_fir_out;
+    for (int k = 0; k < tracks; ++k) {
+        const int grid = conv_frame_ovs(plan->fft_size, album[k].layout.target_piece) == 4 ? 1 : 0;
+        if (leader[grid] < 0) {
+            leader[grid] = k;
+            MGB_TRY(launch_design_fir(*plan, r.design, r.design_stride, grid ? 4 : 2, r.h[grid][0], r.h[grid][1], fir_out,
+                                      album[k].state, st));
+            fir_out = nullptr;
+        }
+    }
+    // stage 2: every track convolved with the album's FIR
+    for (int k = 0; k < tracks; ++k) {
+        const int grid = conv_frame_ovs(plan->fft_size, album[k].layout.target_piece) == 4 ? 1 : 0;
+        if (leader[grid] != k) {
+            float* dst = &album[k].state->fir_peak_mid_bits;
+            const float* src = &album[leader[grid]].state->fir_peak_mid_bits;
+#ifdef MGB_EMULATE
+            memcpy(dst, src, 2 * sizeof(float));
+#else
+            if (cudaMemcpyAsync(dst, src, 2 * sizeof(float), cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+                return cuda_status("album: FIR peaks");
+#endif
+        }
+        Workspace ws = album[k].ws;
+        ws.h_mid = r.h[grid][0];
+        ws.h_side = r.h[grid][1];
+        MGB_TRY(launch_convolve(*plan, album[k].layout, (const float2*)t[k].d_target_lr, (float2*)t[k].d_result_lr, ws,
+                                album[k].state, st));
+    }
+    // stage 3: one launch per step over the whole album
+    for (int step = 1; step < plan->rms_correction_steps; ++step)
+        MGB_TRY(launch_album_loud_sumsq(*plan, album.data(), tracks, step, st));
+    return launch_album_correction_final(*plan, album.data(), tracks, st);
+}
+
 int mgb_correct_levels(const mgb_plan* plan, const mgb_track_layout* L, void* d_workspace, mgb_track_state* d_state,
                        void* stream) {
     MGB_TRY(check_plan(plan));

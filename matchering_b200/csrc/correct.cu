@@ -116,6 +116,132 @@ correction_final_kernel(const double* __restrict__ last_sums, int divisions, lon
     }
 }
 
+// ---- album mastering: the correction steps pooled over the album's tracks (mgb_album_match) --------------------------
+// The album's pieces in track order form one list of G pieces; correction_coefficient runs over it with each lane
+// taking the pieces g = lane (mod 32) in increasing order, so a one-track album adds in the single job's order.
+struct AlbumCorrectTrack {
+    LoudList loud;
+    double* piece_sums;       // [MGB_MAX_CORRECTION_STEPS][div]
+    mgb_track_state* state;
+    long long piece;
+    int div, first_piece;     // the track's pieces are album pieces first_piece .. first_piece + div - 1
+};
+struct AlbumCorrectTable {
+    AlbumCorrectTrack t[MGB_MAX_ALBUM_TRACKS];
+    int count, pieces;
+};
+
+__device__ __forceinline__ double album_correction_coefficient(const AlbumCorrectTable& tab, int row, double eps,
+                                                               double reference_match_rms) {
+    const int lane = threadIdx.x & 31;
+    double acc = 0.0;
+    for (int t = 0; t < tab.count; ++t) {
+        const AlbumCorrectTrack& tr = tab.t[t];
+        const double* sums = tr.piece_sums + (long long)row * tr.div;
+        for (int p = (lane - tr.first_piece) & 31; p < tr.div; p += 32) acc += sums[p] / (double)tr.piece;
+    }
+    const double avg = sqrt(warp_sum(acc) / (double)tab.pieces);
+    double accm = 0.0, cnt = 0.0;
+    for (int t = 0; t < tab.count; ++t) {
+        const AlbumCorrectTrack& tr = tab.t[t];
+        const double* sums = tr.piece_sums + (long long)row * tr.div;
+        for (int p = (lane - tr.first_piece) & 31; p < tr.div; p += 32) {
+            const double r = sqrt(sums[p] / (double)tr.piece);
+            if (r >= avg) {
+                accm += r * r;
+                cnt += 1.0;
+            }
+        }
+    }
+    const double tm = warp_sum(accm);
+    const double tc = warp_sum(cnt);
+    return reference_match_rms / fmax(eps, sqrt(tm / tc));
+}
+
+// loud_sumsq_kernel over every piece of the album: grid = (chunks per piece, album pieces); the prologue's coefficient
+// comes from all tracks' previous-step sums, the rest is the single job's kernel on the piece's own track.
+__global__ void __launch_bounds__(256)
+album_loud_sumsq_kernel(const __grid_constant__ AlbumCorrectTable tab, int step, double eps) {
+    __shared__ double red[32];
+    const int g = blockIdx.y;
+    int t = 0;
+    while (t + 1 < tab.count && tab.t[t + 1].first_piece <= g) ++t;
+    const AlbumCorrectTrack& tr = tab.t[t];
+    const LoudList& loud = tr.loud;
+    const long long p = g - tr.first_piece;
+    const long long piece = tr.piece;
+    mgb_track_state* state = tr.state;
+    const long long n = loud.count[p];
+    const bool fits = n <= loud.capacity;
+    const long long n4 = fits ? (n + 3) / 4 : 0;
+    const long long per4 = (n4 + gridDim.x - 1) / gridDim.x;
+    const long long lo4 = (long long)blockIdx.x * per4;
+    const long long hi4 = lo4 + per4 < n4 ? lo4 + per4 : n4;
+    const float4* row = reinterpret_cast<const float4*>(loud.values + p * loud.capacity);
+    long long i = lo4 + threadIdx.x;
+    float4 v = i < hi4 ? row[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+
+    const double c_prev = album_correction_coefficient(tab, step - 1, eps, state->reference_match_rms);
+    double gain = c_prev;
+    for (int j = 0; j < step - 1; ++j) gain *= state->correction[j];
+    if (blockIdx.x == 0 && p == 0 && threadIdx.x == 0) {
+        state->correction[step - 1] = c_prev;  // no CTA of this launch reads this slot
+        state->steps_done = step;
+    }
+    const float gain_f = (float)gain;
+    double acc = 0.0;
+    if (fits && gain * (double)kLoudMid <= 1.0 - kLoudMargin) {
+        double loud_g = 0.0, loud_1 = 0.0;
+        while (i < hi4) {
+            float4 w = v;
+            const long long e = 4 * i;
+            i += blockDim.x;
+            if (i < hi4) v = row[i];
+            if (e + 1 >= n) w.y = 0.0f;
+            if (e + 2 >= n) w.z = 0.0f;
+            if (e + 3 >= n) w.w = 0.0f;
+            loud_g += clip_sq4(w, gain_f);
+            loud_1 += clip_sq4(w, 1.0f);
+        }
+        acc = loud_g - gain * gain * loud_1;
+        if (blockIdx.x == 0 && threadIdx.x == 0) acc += gain * gain * tr.piece_sums[p];
+    } else {
+        const float2* res = *loud.result_slot;
+        const long long per = (piece + gridDim.x - 1) / gridDim.x;
+        const long long lo = p * piece + (long long)blockIdx.x * per;
+        const long long hi = lo + per < (p + 1) * piece ? lo + per : (p + 1) * piece;
+#pragma unroll 4
+        for (long long f = lo + threadIdx.x; f < hi; f += blockDim.x) {
+            const float2 x = res[f];
+            acc += clip_sq((x.x + x.y) * 0.5f, gain_f);
+        }
+    }
+    const double total = block_sum(acc, red);
+    if (threadIdx.x == 0 && total != 0.0) atomicAdd(&tr.piece_sums[(long long)step * tr.div + p], total);
+}
+
+// correction_final_kernel for every track: CTA t closes track t's chain with the album's last coefficient
+__global__ void __launch_bounds__(32)
+album_correction_final_kernel(const __grid_constant__ AlbumCorrectTable tab, int steps, double eps, double threshold) {
+    mgb_track_state* state = tab.t[blockIdx.x].state;
+    double gain = 1.0;
+    if (steps > 0) {
+        const double c_last = album_correction_coefficient(tab, steps - 1, eps, state->reference_match_rms);
+        gain = c_last;
+        for (int j = 0; j < steps - 1; ++j) gain *= state->correction[j];
+        if (threadIdx.x == 0) state->correction[steps - 1] = c_last;
+    }
+    if (threadIdx.x == 0) {
+        state->steps_done = steps;
+        state->gain = gain;
+        const double peak = (double)state->conv_peak_bits * gain;
+        state->result_peak = peak;
+        state->normalize_coef = fmax(eps, peak / threshold);
+        const double r = fmax(peak, threshold) / threshold;
+        state->limiter_engaged = (fabs(r - 1.0) <= 1e-8 + 1e-5) ? 0 : 1;
+    }
+}
+
 // out = in * gain / divisor, two frames per thread
 __global__ void __launch_bounds__(256)
 scale_kernel(const float4* __restrict__ in, float4* __restrict__ out, long long pairs, const float2* __restrict__ in_tail,
@@ -329,6 +455,42 @@ int launch_correction_final(const mgb_plan& plan, const mgb_track_layout& layout
     const double* last = ws.piece_sums + (long long)(steps > 0 ? steps - 1 : 0) * div;
     return launch("correction_final_kernel", correction_final_kernel, dim3(1), dim3(32), 0, stream, last, div,
                   (long long)layout.target_piece, steps, plan.min_value, plan.threshold, state);
+}
+
+static AlbumCorrectTable album_correct_table(const AlbumTrack* tracks, int count) {
+    AlbumCorrectTable tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.count = count;
+    for (int t = 0; t < count; ++t) {
+        const Workspace& ws = tracks[t].ws;
+        AlbumCorrectTrack& d = tab.t[t];
+        d.loud = LoudList{ws.loud_values, ws.loud_count, (long long)ws.loud_capacity, ws.result_slot};
+        d.piece_sums = ws.piece_sums;
+        d.state = tracks[t].state;
+        d.piece = tracks[t].layout.target_piece;
+        d.div = tracks[t].layout.target_divisions;
+        d.first_piece = tab.pieces;
+        tab.pieces += d.div;
+    }
+    return tab;
+}
+
+int launch_album_loud_sumsq(const mgb_plan& plan, const AlbumTrack* tracks, int count, int step, cudaStream_t stream) {
+    // launch_loud_sumsq's grid over the album's pieces, sized for its longest piece
+    const AlbumCorrectTable tab = album_correct_table(tracks, count);
+    long long longest = 0;
+    for (int t = 0; t < count; ++t) longest = tracks[t].layout.target_piece > longest ? tracks[t].layout.target_piece : longest;
+    long long per_piece = (3LL * num_sms() + tab.pieces - 1) / tab.pieces;
+    const long long max_useful = (longest + 8191) / 8192;
+    if (per_piece > max_useful) per_piece = max_useful;
+    if (per_piece < 1) per_piece = 1;
+    return launch("album_loud_sumsq_kernel", album_loud_sumsq_kernel, dim3((unsigned)per_piece, (unsigned)tab.pieces),
+                  dim3(256), 0, stream, tab, step, plan.min_value);
+}
+
+int launch_album_correction_final(const mgb_plan& plan, const AlbumTrack* tracks, int count, cudaStream_t stream) {
+    return launch("album_correction_final_kernel", album_correction_final_kernel, dim3((unsigned)count), dim3(32), 0, stream,
+                  album_correct_table(tracks, count), plan.rms_correction_steps, plan.min_value, plan.threshold);
 }
 
 int launch_scale(const float2* in, float2* out, int64_t frames, const double* gain, const double* divisor,

@@ -787,6 +787,189 @@ smooth_operator_kernel(const double* __restrict__ S, const int4* __restrict__ ro
     }
 }
 
+// ---- album mastering: spectrum_mean_kernel's profiled half pooled over the tracks of an album -------------------------
+// (mgb_album_match; DESIGN.md section 4 "Album mastering").  The tracks travel as a kernel parameter: no copy on the
+// stream, no table in a workspace.
+struct AlbumMeanTrack {
+    const float* spec_part;    // [D][S][2][n_lin] the track's analysis partials
+    const double* sumsq_part;  // [D][S]
+    const float* absmax_part;  // [D*S + 1]
+    unsigned char* mask;       // [D] out: the track's pieces in the album's loud mask
+    float* target_peak;        // out: the track's own peak (its convolution's choice of precision)
+    mgb_track_state* state;    // out: the album's level statistics
+    long long piece, frames_per_piece;
+    int div, slots;
+};
+struct AlbumMeanTable {
+    AlbumMeanTrack t[MGB_MAX_ALBUM_TRACKS];
+    int count;
+};
+
+// The album's pieces in track order are one list of G = sum D_t pieces; everything the single-track kernel does per
+// piece and per (piece, slot) item runs over that list in the same order, so a one-track album is the profiled job
+// bit for bit.  grid = (ceil(n_lin/32), 2), as spectrum_mean_kernel.
+__global__ void __launch_bounds__(kMeanBins * kMeanSlices)
+album_mean_kernel(const __grid_constant__ AlbumMeanTable tab, const mgb_reference_profile* __restrict__ profile,
+                  double* __restrict__ scratch, long long stride, int n_lin, int fft_size, double eps, PrefetchList pf) {
+    constexpr int BINS = kMeanBins, SLICES = kMeanSlices;
+    __shared__ double part_t[SLICES][BINS + 1];
+    __shared__ int piece_off[MGB_MAX_ALBUM_TRACKS + 1], sel_off[MGB_MAX_ALBUM_TRACKS + 1];
+    __shared__ LevelsResult lv_s;
+    __shared__ long long frames_s;  // boxcar frames of the loud pieces of every track
+    MGB_DYN_SMEM(smem);
+    const int K = tab.count;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    {
+        const long long gtid = ((long long)blockIdx.y * gridDim.x + blockIdx.x) * blockDim.x + threadIdx.x;
+        const long long gsize = (long long)gridDim.x * gridDim.y * blockDim.x;
+        for (int t = 0; t < pf.count; ++t)
+            for (long long off = gtid * 128; off < pf.bytes[t]; off += gsize * 128)
+                prefetch_l2(reinterpret_cast<const char*>(pf.ptr[t]) + off);
+    }
+    if (threadIdx.x == 0) {
+        piece_off[0] = 0;
+        for (int t = 0; t < K; ++t) piece_off[t + 1] = piece_off[t] + tab.t[t].div;
+    }
+    __syncthreads();
+    const int G = piece_off[K];
+    auto track_of = [&](int g) {
+        int t = 0;
+        while (piece_off[t + 1] <= g) ++t;
+        return t;
+    };
+    unsigned char* mask = smem;                                                   // [G]
+    double* piece_sum = reinterpret_cast<double*>(smem + (G + 15) / 16 * 16);     // [G]
+    int* piece_rank = reinterpret_cast<int*>(piece_sum + G);                      // [G]
+    unsigned* sel = reinterpret_cast<unsigned*>(piece_rank + (G + 1) / 2 * 2);    // [sum of items]: track << 16 | item
+    if (blockIdx.x == 0 && blockIdx.y == 0) {  // each track's own peak, for its convolution
+        for (int t = warp; t < K; t += nwarps) {
+            float tpk = 0.0f;
+            for (int i = lane; i < tab.t[t].div * tab.t[t].slots + 1; i += 32) tpk = fmaxf(tpk, tab.t[t].absmax_part[i]);
+            tpk = warp_max_f(tpk);
+            if (lane == 0) *tab.t[t].target_peak = tpk;
+        }
+    }
+    for (int g = warp; g < G; g += nwarps) {
+        const int t = track_of(g);
+        const int slots = tab.t[t].slots;
+        const double* part = tab.t[t].sumsq_part + (long long)(g - piece_off[t]) * slots;
+        double sum = 0.0;
+        for (int k = lane; k < slots; k += 32) sum += part[k];
+        sum = warp_sum(sum);
+        if (lane == 0) piece_sum[g] = sum;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        // signal_levels_warp over the album's pieces, each with its own track's piece length
+        double acc = 0.0;
+        for (int g = lane; g < G; g += 32) {
+            const double r = sqrt(piece_sum[g] / (double)tab.t[track_of(g)].piece);
+            acc += r * r;
+        }
+        const double avg = sqrt(warp_sum(acc) / (double)G);
+        double accm = 0.0, cnt = 0.0;
+        for (int g = lane; g < G; g += 32) {
+            const double r = sqrt(piece_sum[g] / (double)tab.t[track_of(g)].piece);
+            const bool m = r >= avg;
+            mask[g] = m ? 1 : 0;
+            if (m) {
+                accm += r * r;
+                cnt += 1.0;
+            }
+        }
+        const double tm = warp_sum(accm);
+        const double tc = warp_sum(cnt);
+        LevelsResult mine;
+        mine.peak = profile->reference_peak;
+        mine.coef = profile->final_amplitude_coef;
+        mine.match_t = sqrt(tm / tc);
+        mine.match_r = profile->reference_match_rms;
+        mine.c0 = mine.match_r / fmax(eps, mine.match_t);
+        mine.loud_t = (int)tc;
+        mine.loud_r = profile->reference_loud_pieces;
+        __syncwarp();
+        // each track's loud pieces ranked as spectrum_mean_kernel ranks one signal's; the album's item list is the
+        // tracks' lists one after another
+        int items = 0;
+        long long frames = 0;
+        for (int t = 0; t < K; ++t) {
+            const int div = tab.t[t].div, off = piece_off[t];
+            int count = 0;
+            for (int base_p = 0; base_p < div; base_p += 32) {
+                const int p = base_p + lane;
+                const bool keep = p < div && mask[off + p];
+                const unsigned votes = __ballot_sync(0xffffffffu, keep);
+                if (p < div) piece_rank[off + p] = count + __popc(votes & ((1u << lane) - 1u));
+                count += __popc(votes);
+            }
+            if (lane == 0) sel_off[t] = items;
+            items += count * tab.t[t].slots;
+            frames += (long long)count * tab.t[t].frames_per_piece;
+        }
+        if (lane == 0) {
+            sel_off[K] = items;
+            frames_s = frames;
+            lv_s = mine;
+        }
+    }
+    __syncthreads();
+    const LevelsResult lv = lv_s;
+    if (blockIdx.x == 0 && blockIdx.y == 0) {
+        if (threadIdx.x < K) {
+            mgb_track_state* st = tab.t[threadIdx.x].state;
+            levels_store(lv, st);
+            st->conv_peak_bits = 0.0f;
+            st->fir_peak_mid_bits = 0.0f;
+            st->fir_peak_side_bits = 0.0f;
+            st->conv_precise = 0;
+        }
+        for (int g = threadIdx.x; g < G; g += blockDim.x) {
+            const int t = track_of(g);
+            tab.t[t].mask[g - piece_off[t]] = mask[g];
+        }
+    }
+    for (int t = 0; t < K; ++t) {  // every thread files its share of each track's items: piece by piece, slot by slot
+        const int slots = tab.t[t].slots, off = piece_off[t];
+        const int items = tab.t[t].div * slots;
+        unsigned* out = sel + sel_off[t];
+        for (int it = threadIdx.x; it < items; it += blockDim.x) {
+            const int p = it / slots;
+            if (mask[off + p]) out[piece_rank[off + p] * slots + (it - p * slots)] = ((unsigned)t << 16) | (unsigned)it;
+        }
+    }
+    __syncthreads();
+    const int bx = threadIdx.x % BINS, sy = threadIdx.x / BINS;
+    const int k = blockIdx.x * BINS + bx;
+    const int ch = blockIdx.y;
+    double st = 0.0;
+    if (k < n_lin) {
+        const int count = sel_off[K];
+        for (int i = sy; i < count; i += 8 * SLICES) {
+            float v[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+                const int iu = i + u * SLICES;
+                float x = 0.0f;
+                if (iu < count) {
+                    const unsigned e = sel[iu];
+                    x = tab.t[e >> 16].spec_part[((long long)(e & 0xffffu) * 2 + ch) * n_lin + k];
+                }
+                v[u] = x;
+            }
+            st += (((double)v[0] + (double)v[1]) + ((double)v[2] + (double)v[3])) +
+                  (((double)v[4] + (double)v[5]) + ((double)v[6] + (double)v[7]));
+        }
+    }
+    part_t[sy][bx] = st;
+    __syncthreads();
+    if (sy == 0 && k < n_lin) {
+        for (int q = 1; q < SLICES; ++q) st += part_t[q][bx];
+        const double norm_t = lv.c0 / ((double)frames_s * (double)fft_size);
+        const double* spectra = reinterpret_cast<const double*>(profile + 1);
+        scratch[(long long)(kDesignBlocks * ch) * stride + k] = spectra[(long long)ch * n_lin + k] / fmax(eps, st * norm_t);
+    }
+}
+
 // dynamic shared memory of spectrum_mean_kernel: both masks, the per-piece sums and the two item lists
 size_t spectrum_mean_smem(int div_t, int64_t items_t, int div_r, int64_t items_r) {
     return (size_t)((div_t + div_r + 15) / 16 * 16 + (int64_t)(div_t + div_r) * 8 + (items_t + items_r) * 2 + 16);
@@ -795,6 +978,20 @@ size_t spectrum_mean_smem(int div_t, int64_t items_t, int div_r, int64_t items_r
 template <int F>
 int launch_design_t(const mgb_plan& plan, const DesignArgs& a, cudaStream_t stream) {
     return launch("design_kernel", design_kernel<F>, dim3(2 * a.ovs), dim3(kDesignThreads), DesignSmem<F>::kBytes, stream, plan, a);
+}
+
+int launch_design_kernel(const mgb_plan& plan, const DesignArgs& a, cudaStream_t stream) {
+    switch (plan.fft_size) {
+        case 512: return launch_design_t<512>(plan, a, stream);
+        case 1024: return launch_design_t<1024>(plan, a, stream);
+        case 2048: return launch_design_t<2048>(plan, a, stream);
+        case 4096: return launch_design_t<4096>(plan, a, stream);
+        case 8192: return launch_design_t<8192>(plan, a, stream);
+        case 16384: return launch_design_t<16384>(plan, a, stream);
+        default: break;
+    }
+    set_error("design: fft_size %d has no kernel", plan.fft_size);
+    return MGB_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -913,17 +1110,7 @@ int launch_design(const mgb_plan& plan, const mgb_track_layout& layout, const Wo
                        plan.d_smooth_op, (const int4*)plan.d_smooth_op_rows, a.scratch, a.stride, plan.n_lin));
         a.s_ready = 1;
     }
-    switch (plan.fft_size) {
-        case 512: return launch_design_t<512>(plan, a, stream);
-        case 1024: return launch_design_t<1024>(plan, a, stream);
-        case 2048: return launch_design_t<2048>(plan, a, stream);
-        case 4096: return launch_design_t<4096>(plan, a, stream);
-        case 8192: return launch_design_t<8192>(plan, a, stream);
-        case 16384: return launch_design_t<16384>(plan, a, stream);
-        default: break;
-    }
-    set_error("design: fft_size %d has no kernel", plan.fft_size);
-    return MGB_ERR_UNSUPPORTED;
+    return launch_design_kernel(plan, a, stream);
 }
 
 int launch_design_native(const mgb_plan& plan, const Workspace& ws, const mgb_plan& nplan, const mgb_track_layout& nlayout,
@@ -994,6 +1181,84 @@ int launch_reference_profile(const mgb_plan& plan, const ReferenceGeometry& g, c
                   dim3((plan.n_lin + kMeanBins - 1) / kMeanBins, 2), dim3(kMeanBins * kMeanSlices),
                   spectrum_mean_smem(0, 0, g.divisions, (int64_t)g.divisions * g.slots), stream, a, plan.n_lin, plan.fft_size,
                   plan.min_value, pf, io);
+}
+
+size_t album_mean_smem(const AlbumTrack* tracks, int count) {
+    int64_t pieces = 0, items = 0;
+    for (int t = 0; t < count; ++t) {
+        pieces += tracks[t].layout.target_divisions;
+        items += (int64_t)tracks[t].layout.target_divisions * tracks[t].layout.target_slots;
+    }
+    return (size_t)((pieces + 15) / 16 * 16 + pieces * 8 + (pieces + 1) / 2 * 8 + items * 4 + 16);
+}
+
+int launch_album_mean(const mgb_plan& plan, const AlbumTrack* tracks, int count, const mgb_reference_profile* profile,
+                      double* design, int64_t design_stride, cudaStream_t stream) {
+    AlbumMeanTable tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.count = count;
+    for (int t = 0; t < count; ++t) {
+        const mgb_track_layout& L = tracks[t].layout;
+        const Workspace& ws = tracks[t].ws;
+        AlbumMeanTrack& d = tab.t[t];
+        d.spec_part = ws.spec_part_t;
+        d.sumsq_part = ws.sumsq_part_t;
+        d.absmax_part = ws.absmax_part_t;
+        d.mask = ws.mask_t;
+        d.target_peak = ws.target_peak;
+        d.state = tracks[t].state;
+        d.piece = L.target_piece;
+        d.frames_per_piece = L.target_piece / plan.fft_size;
+        d.div = L.target_divisions;
+        d.slots = L.target_slots;
+    }
+    // (the design kernels' tables, pulled back into L2 as spectrum_mean_kernel does)
+    PrefetchList pf;
+    memset(&pf, 0, sizeof(pf));
+    auto add = [&](const void* p, long long bytes) {
+        if (p && pf.count < 14) {
+            pf.ptr[pf.count] = p;
+            pf.bytes[pf.count] = bytes;
+            pf.count++;
+        }
+    };
+    const long long nl = plan.n_lin, ng = plan.n_log;
+    add(plan.d_sa_hinv, (nl - 1) * 8);
+    add(plan.d_sa_lu, 3 * (nl - 2) * 8);
+    add(plan.d_sa_eval_idx, ng * 4);
+    add(plan.d_sa_eval_w, ng * 32);
+    add(plan.d_sb_hinv, (ng - 1) * 8);
+    add(plan.d_sb_lu, 3 * (ng - 2) * 8);
+    add(plan.d_sb_eval_idx, nl * 4);
+    add(plan.d_sb_eval_w, nl * 32);
+    add(plan.d_lw_fit_left, (long long)plan.lowess_nfit * 4);
+    add(plan.d_lw_row_idx, (long long)plan.lowess_nfit * 4);
+    add(plan.d_lw_seg, ng * 4);
+    add(plan.d_lw_alpha, ng * 8);
+    add(plan.d_lw_rows, (long long)plan.lowess_nrows * plan.lowess_k * 8);
+    add(plan.d_hann, (long long)plan.fft_size * 8);
+    return launch("album_mean_kernel", album_mean_kernel, dim3((plan.n_lin + kMeanBins - 1) / kMeanBins, 2),
+                  dim3(kMeanBins * kMeanSlices), album_mean_smem(tracks, count), stream, tab, profile, design,
+                  (long long)design_stride, plan.n_lin, plan.fft_size, plan.min_value, pf);
+}
+
+int launch_design_fir(const mgb_plan& plan, double* design, int64_t design_stride, int ovs, float2* h_mid, float2* h_side,
+                      double* fir_out, mgb_track_state* state, cudaStream_t stream) {
+    DesignArgs a;
+    memset(&a, 0, sizeof(a));
+    a.scratch = design;
+    a.stride = design_stride;
+    a.fir_out = fir_out;
+    a.h_mid = h_mid;
+    a.h_side = h_side;
+    a.state = state;
+    a.ovs = ovs;
+    if (plan.d_smooth_op && plan.d_smooth_op_rows) {
+        MGB_TRY(launch("smooth_operator_kernel", smooth_operator_kernel, dim3((plan.n_lin + 3) / 4), dim3(128), 0, stream,
+                       plan.d_smooth_op, (const int4*)plan.d_smooth_op_rows, a.scratch, a.stride, plan.n_lin));
+        a.s_ready = 1;
+    }
+    return launch_design_kernel(plan, a, stream);
 }
 
 }  // namespace mgb

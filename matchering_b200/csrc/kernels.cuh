@@ -133,6 +133,25 @@ int64_t operator_workspace_bytes(const mgb_plan& plan);
 int build_operator(const mgb_plan& plan, double* op_out, void* workspace, cudaStream_t stream);
 extern int g_design_direct;  // tests: force the direct (non-operator) smoothing in mgb_test_design_fir
 
+// album mastering (mgb_album_match): one entry per track, in album order
+struct AlbumTrack {
+    mgb_track_layout layout;
+    Workspace ws;
+    mgb_track_state* state;
+};
+// design.cu: the pooled level statistics and target spectra of the album into every track's state, mask and target peak,
+// and the matching curve into `design` (a job's design blocks); then launch_design_fir
+size_t album_mean_smem(const AlbumTrack* tracks, int count);
+int launch_album_mean(const mgb_plan& plan, const AlbumTrack* tracks, int count, const mgb_reference_profile* profile,
+                      double* design, int64_t design_stride, cudaStream_t stream);
+// the smoothing and design_kernel over a matching curve already in `design`: FIR spectra on the ovs*F grid into
+// h_mid / h_side, their peaks into *state
+int launch_design_fir(const mgb_plan& plan, double* design, int64_t design_stride, int ovs, float2* h_mid, float2* h_side,
+                      double* fir_out, mgb_track_state* state, cudaStream_t stream);
+// correct.cu: RMS-correction step `step` (1 .. steps-1) and the closing kernel, pooled over the album, one launch each
+int launch_album_loud_sumsq(const mgb_plan& plan, const AlbumTrack* tracks, int count, int step, cudaStream_t stream);
+int launch_album_correction_final(const mgb_plan& plan, const AlbumTrack* tracks, int count, cudaStream_t stream);
+
 // convolve.cu -----------------------------------------------------------------------------------
 int conv_frame_ovs(int fft_size, long long target_piece);  // 2 or 4: transform length of the convolution in FIR lengths
 int launch_convolve(const mgb_plan& plan, const mgb_track_layout& layout, const float2* target, float2* result,

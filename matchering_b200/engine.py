@@ -245,6 +245,26 @@ class TrackSession:
         return _native.TrackState.from_buffer_copy(raw)
 
 
+def album_match(sessions: list, targets: list, d_profile: torch.Tensor, fir_out: torch.Tensor | None = None) -> None:
+    """Stages 1-3 of an album (mgb_album_match): one TrackSession per track, each a profiled session of the same plan,
+    and its target on the device.  Leaves every session where correct_levels leaves a single job."""
+    plan = sessions[0].plan
+    n = len(sessions)
+    table = (_native.AlbumTrack * n)()
+    for entry, session, target in zip(table, sessions, targets):
+        entry.layout = C.pointer(session.layout)
+        entry.d_target_lr, entry.d_result_lr = target.data_ptr(), session.result.data_ptr()
+        entry.d_workspace, entry.d_state = session.workspace.data_ptr(), session.state.data_ptr()
+    layouts = (_native.TrackLayout * n)(*(s.layout for s in sessions))
+    ws_bytes = int(plan.lib.mgb_album_workspace_bytes(C.byref(plan.struct), n, layouts))
+    if ws_bytes < 0:
+        raise ValueError(plan.lib.mgb_last_error_string().decode("utf-8", "replace"))
+    album_ws = torch.empty(ws_bytes, dtype=torch.uint8, device=plan.device)
+    _native.check(plan.lib, plan.lib.mgb_album_match(
+        C.byref(plan.struct), n, table, d_profile.data_ptr(), fir_out.data_ptr() if fir_out is not None else None,
+        album_ws.data_ptr(), ws_bytes, _stream_ptr(plan.device)))
+
+
 # ------------------------------------------------------------------------------------------------
 # host arrays in, host arrays out (the reference's seam: pageable float64 numpy, core.py:77-86)
 # ------------------------------------------------------------------------------------------------

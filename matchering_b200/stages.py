@@ -7,8 +7,8 @@ import torch
 
 from . import _native, plan as _plan
 from .defaults import Config
-from .engine import (TrackSession, get_native_plan, get_plan, host_array_ok, stages_main_host, stages_main_host_profiled,
-                     to_device_f32, to_host_like)
+from .engine import (TrackSession, album_match, get_native_plan, get_plan, host_array_ok, stages_main_host,
+                     stages_main_host_profiled, to_device_f32, to_host_like)
 from .log import Code, info, debug, debug_line, debug_enabled
 from .profile import ReferenceProfile
 from .utils import to_db
@@ -215,3 +215,68 @@ def main_native_device(target, sample_rate: int, reference, config: Config, need
                                                         _native.LoudnessTargetReport.from_buffer_copy(raw)))
 
     return limited, plain, normalized
+
+
+def main_album(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
+               need_no_limiter_normalized: bool = False):
+    """Master the K tracks of an album against one reference with ONE level match and ONE matching FIR, from
+    statistics pooled over every piece of every track (DESIGN.md section 4 "Album mastering"), so the tracks keep their
+    relative levels and share one tonal correction.  targets: a list of (N_t, 2) stereo arrays at
+    config.internal_sample_rate, numpy or torch; reference: samples or a ReferenceProfile.  Returns one
+    (result, result_no_limiter, result_no_limiter_normalized) per track, None where not requested, in each target's
+    array type.  The normalized result is normalised per track, as in `main`.  A one-track album is `main` with the
+    reference's profile, bit for bit."""
+    outs = main_album_device(targets, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
+    return [tuple(None if t is None else to_host_like(t, target) for t in track) for track, target in zip(outs, targets)]
+
+
+def album_check(count: int, config: Config) -> None:
+    """The album requests main_album refuses before any device work."""
+    if count < 1:
+        raise ValueError("an album needs at least one track")
+    if count > _native.MGB_MAX_ALBUM_TRACKS:
+        raise ValueError(f"an album of {count} tracks: at most {_native.MGB_MAX_ALBUM_TRACKS} are mastered together")
+    if config.loudness_target is not None:
+        raise ValueError("Config(loudness_target=...) is not available for albums: a target per track would undo the "
+                         "album's level relation")
+
+
+def main_album_device(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
+                      need_no_limiter_normalized: bool = False, fir_out=None):
+    """`main_album` with the results left on the device as float32 CUDA tensors.  fir_out: optional (2, fft_size)
+    float64 CUDA tensor that receives the album's mid and side FIRs."""
+    targets = list(targets)
+    album_check(len(targets), config)
+    for target in targets:
+        if target.ndim != 2 or target.shape[1] != 2:
+            raise ValueError("every target must be a (frames, 2) stereo array")
+        if not target.shape[0] > config.fft_size:
+            raise ValueError(f"every target must be longer than fft_size ({config.fft_size} frames)")
+    if not isinstance(reference, ReferenceProfile):
+        from .profile import analyze_reference
+        reference = analyze_reference(reference, config)
+    reference.check_config(config)
+    plan = get_plan(config)
+    device = plan.device
+    with torch.cuda.device(device):
+        d_profile = reference.checked_blob(plan)
+        d_targets = [to_device_f32(t, device) for t in targets]
+        sessions = [TrackSession(plan, int(t.shape[0]), None) for t in d_targets]
+
+        debug_line()
+        info(Code.INFO_MATCHING_LEVELS)
+        debug(f"Album of {len(sessions)} tracks, pieces per track: {[int(s.layout.target_divisions) for s in sessions]}")
+        info(Code.INFO_MATCHING_FREQS)
+        info(Code.INFO_CORRECTING_LEVELS)
+        album_match(sessions, d_targets, d_profile, fir_out)
+
+        debug_line()
+        info(Code.INFO_FINALIZING)
+        outs = [s.finalize(need_default, need_no_limiter, need_no_limiter_normalized) for s in sessions]
+        if debug_enabled():
+            st = sessions[0].read_state()
+            debug(f"The album's {st.target_loud_pieces} loud pieces of {sum(int(s.layout.target_divisions) for s in sessions)}"
+                  f" give one RMS coefficient: {to_db(st.rms_coefficient)}")
+            for step in range(st.steps_done):
+                debug(f"Album RMS correction #{step + 1}: {to_db(st.correction[step])}")
+    return outs
