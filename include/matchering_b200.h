@@ -453,6 +453,37 @@ int mgb_limit_to_loudness(const mgb_limiter_params* params, const mgb_loudness_p
                           const float* d_in_lr, float* d_out_lr, int64_t frames, void* d_workspace, int64_t workspace_bytes,
                           mgb_loudness_target_report* d_report, void* stream);
 
+/* ---- album loudness: an album metered as one programme, and driven to a target with one drive (DESIGN.md section 4) --
+ * The album meter: each of the K tracks is K-weighted from rest and cut into its own sub-blocks and windows, exactly as
+ * mgb_loudness does; no window straddles two tracks.  The album's integrated loudness and loudness range are then
+ * mgb_loudness's gates and percentiles over the union of all tracks' windows (every window counts once), and its
+ * maxima and peaks the maxima over the tracks (libebur128's ebur128_loudness_global_multiple / _range_multiple).  It is
+ * not the meter of the tracks concatenated.  A one-track album is mgb_loudness bit for bit. */
+int64_t mgb_album_loudness_workspace_bytes(const mgb_loudness_params* params, int32_t tracks, const int64_t* frames);
+/* d_lr[t]: frames[t] stereo frames per track (host arrays of device pointers).  *d_album_result: the album's result,
+ * its momentary_count / short_term_count the pooled counts.  d_track_results (optional, device, [tracks]): each
+ * track's own mgb_loudness result.  MGB_ERR_INVALID: no tracks or more than MGB_MAX_ALBUM_TRACKS, a track without
+ * frames, NULL or misaligned pointers; MGB_ERR_WORKSPACE: a short workspace.  The workspace needs no initialisation. */
+int mgb_album_loudness(const mgb_loudness_params* params, int32_t tracks, const float* const* d_lr, const int64_t* frames,
+                       void* d_workspace, int64_t workspace_bytes, mgb_loudness_result* d_album_result,
+                       mgb_loudness_result* d_track_results, void* stream);
+/* The album target, after mgb_album_match: s_t = result_t * gain (the album's correction gain, the same in every
+ * track), y_t(x) = limit_t(s_t * 10^(x/20)) with each track's own limiter in the plan's peak mode and no
+ * final_amplitude_coefficient, and ONE drive x for every track, searched by mgb_finalize_to_loudness's rule with I the
+ * album meter's integrated loudness of y_1(x) .. y_K(x).  Where no limiter engages the tracks keep their relative levels
+ * exactly.  d_out_limited[t] (host array of device pointers) receives y_t(x*); it also stages s_t, so it must not be the
+ * track's d_result_lr.  d_report (device): the album's report.  Each track's workspace and state are its
+ * mgb_album_match entry's.  MGB_ERR_INVALID: bad track count, NULL or misaligned pointers, an output that is its track's
+ * result, a layout not of this plan, a meter rate that is not the plan's, a target mgb_finalize_to_loudness rejects;
+ * MGB_ERR_WORKSPACE: a short search workspace.  A one-track album computes what mgb_finalize_to_loudness computes, bit
+ * for bit.  Nothing here synchronises. */
+int64_t mgb_album_loudness_target_workspace_bytes(const mgb_loudness_params* meter, int32_t tracks,
+                                                  const mgb_track_layout* layouts);
+int mgb_album_finalize_to_loudness(const mgb_plan* plan, int32_t tracks, const mgb_album_track* t,
+                                   float* const* d_out_limited, const mgb_loudness_params* meter,
+                                   const mgb_loudness_target* target, void* d_search_ws, int64_t search_ws_bytes,
+                                   mgb_loudness_target_report* d_report, void* stream);
+
 /* ---- whole job with HOST buffers (the call the end-to-end benchmark times) --------------------
  * h_* are host pointers (pinned for full speed).  Copies target and reference to the device,
  * runs stages 1-4 and copies the requested outputs back; synchronises `stream` before returning.

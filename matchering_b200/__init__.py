@@ -13,7 +13,7 @@ from .defaults import Config, LimiterConfig
 from .loader import load
 from .checker import check
 from .profile import ReferenceProfile, analyze_reference
-from .loudness import Loudness, loudness  # (the function shadows the module name on the package)
+from .loudness import AlbumLoudness, Loudness, album_loudness, loudness  # (the function shadows the module name on the package)
 
 
 def process(*args, **kwargs):

@@ -293,6 +293,13 @@ PROTOTYPES = {
                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_limit_to_loudness": (C.c_int, [C.POINTER(LimiterParams), C.POINTER(LoudnessParams), C.POINTER(LoudnessTargetParams),
                                         C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "mgb_album_loudness_workspace_bytes": (C.c_int64, [C.POINTER(LoudnessParams), C.c_int32, C.POINTER(C.c_int64)]),
+    "mgb_album_loudness": (C.c_int, [C.POINTER(LoudnessParams), C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                     C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "mgb_album_loudness_target_workspace_bytes": (C.c_int64, [C.POINTER(LoudnessParams), C.c_int32, C.POINTER(TrackLayout)]),
+    "mgb_album_finalize_to_loudness": (C.c_int, [C.POINTER(Plan), C.c_int32, C.POINTER(AlbumTrack), C.POINTER(C.c_void_p),
+                                                 C.POINTER(LoudnessParams), C.POINTER(LoudnessTargetParams), C.c_void_p,
+                                                 C.c_int64, C.c_void_p, C.c_void_p]),
     "mgb_pipeline_enable_loudness_target": (C.c_int, [C.c_void_p, C.POINTER(LoudnessTargetParams)]),
     "mgb_pipeline_wait_loudness_target": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(TrackState), C.POINTER(LoudnessResult),
                                                     C.POINTER(LoudnessTargetReport)]),

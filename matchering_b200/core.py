@@ -3,7 +3,7 @@ validation and saving are host plumbing; `stages.main` in the middle runs on the
 from .checker import check, check_equality
 from .defaults import Config
 from .loader import load
-from .log import Code, ModuleError, debug, debug_line, info
+from .log import Code, ModuleError, debug, debug_enabled, debug_line, info
 from .profile import ReferenceProfile
 from .results import Result
 from .saver import save
@@ -79,19 +79,20 @@ def process(target: str, reference, results: list, config: Config = None,
     info(Code.INFO_COMPLETED)
 
 
-def process_album(targets: list, reference, results: list, config: Config = None):
+def process_album(targets: list, reference, results: list, config: Config = None, album_loudness_target: float = None):
     """Master an album: `targets` is a list of file paths, `results` a list of the same length whose entries are lists
     of Result as mg.process takes them.  Every target is loaded and checked as mg.process loads its target; then ONE
     level match and ONE matching FIR, from statistics pooled over every track (stages.main_album), master them all, so
     the tracks keep their relative levels.  `reference` is a file path or a ReferenceProfile.  Config(loudness_target=...)
-    and native-rate targets are refused."""
+    and native-rate targets are refused.  album_loudness_target (LUFS): the limited results are driven with ONE limiter
+    gain until the album, metered as one programme (mg.album_loudness), reads that loudness."""
     from .stages import album_check, main_album_device
     if config is None:
         config = Config()
     targets, results = list(targets), list(results)
     if not targets or len(targets) != len(results):
         raise ValueError(f"process_album: {len(targets)} targets and {len(results)} result lists")
-    album_check(len(targets), config)
+    album_check(len(targets), config, album_loudness_target)
     if any(not r for r in results):
         raise ValueError("process_album: every track needs at least one Result")
     if config.native_rate:
@@ -129,7 +130,13 @@ def process_album(targets: list, reference, results: list, config: Config = None
     needs = dict(need_default=any(r.use_limiter for r in everything),
                  need_no_limiter=any(not r.use_limiter and not r.normalize for r in everything),
                  need_no_limiter_normalized=any(not r.use_limiter and r.normalize for r in everything))
-    outs = main_album_device(audios, reference, config, **needs)
+    outs = main_album_device(audios, reference, config, album_loudness_target=album_loudness_target, **needs)
+    if album_loudness_target is not None and needs["need_default"] and debug_enabled():
+        from .loudness import album_loudness
+        m = album_loudness([limited for limited, _, _ in outs], config.internal_sample_rate)
+        debug(f"The album's masters read {m.album.integrated:.4f} LUFS as one programme")
+        for t, (path, track) in enumerate(zip(targets, m.tracks)):
+            debug(f"Master {t + 1} ('{path}'): {track.integrated:.4f} LUFS, true peak {track.true_peak:.2f} dBTP")
     debug_line()
     info(Code.INFO_EXPORTING)
     for (limited, plain, normalized), wanted_list in zip(outs, results):

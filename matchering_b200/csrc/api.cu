@@ -947,6 +947,70 @@ int mgb_finalize_to_loudness(const mgb_plan* plan, const mgb_track_layout* L, co
                                tp ? ws.tp_plane : nullptr, d_search_ws, d_report, st);
 }
 
+int mgb_album_finalize_to_loudness(const mgb_plan* plan, int32_t tracks, const mgb_album_track* t,
+                                   float* const* d_out_limited, const mgb_loudness_params* meter,
+                                   const mgb_loudness_target* target, void* d_search_ws, int64_t search_ws_bytes,
+                                   mgb_loudness_target_report* d_report, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(tracks >= 1 && tracks <= MGB_MAX_ALBUM_TRACKS, MGB_ERR_INVALID, "album loudness target: %d tracks (1 .. %d)",
+                (int)tracks, MGB_MAX_ALBUM_TRACKS);
+    MGB_REQUIRE(t != nullptr && d_out_limited != nullptr, MGB_ERR_INVALID,
+                "album loudness target: the track table or the output table is NULL");
+    MGB_TRY(loudness_target_validate(target, meter));
+    MGB_REQUIRE(meter->sample_rate == plan->sample_rate, MGB_ERR_INVALID,
+                "album loudness target: the meter's rate %d differs from the plan's %d", meter->sample_rate, plan->sample_rate);
+    MGB_REQUIRE(plan->d_limiter_tables != nullptr, MGB_ERR_INVALID, "album loudness target: the plan has no limiter tables");
+    std::vector<mgb_track_layout> layouts((size_t)tracks);
+    for (int k = 0; k < tracks; ++k) {
+        MGB_TRY(check_album_layout(plan, t[k].layout, k));
+        MGB_TRY(check_aligned(t[k].d_result_lr, "d_result_lr"));
+        MGB_TRY(check_aligned(t[k].d_workspace, "d_workspace"));
+        MGB_TRY(check_aligned(t[k].d_state, "d_state"));
+        MGB_TRY(check_aligned(d_out_limited[k], "d_out_limited"));
+        // (s = result * gain is staged in the output while every pass still reads the result)
+        MGB_REQUIRE((const void*)d_out_limited[k] != (const void*)t[k].d_result_lr, MGB_ERR_INVALID,
+                    "album loudness target: track %d: d_out_limited is its d_result_lr (the output is the search's scratch)", k);
+        layouts[k] = *t[k].layout;
+    }
+    MGB_TRY(check_aligned(d_search_ws, "d_search_ws"));
+    MGB_TRY(check_aligned(d_report, "d_report"));
+    const int64_t need = mgb_album_loudness_target_workspace_bytes(meter, tracks, layouts.data());
+    MGB_REQUIRE(search_ws_bytes >= need, MGB_ERR_WORKSPACE, "album loudness target: search workspace of %lld bytes, need %lld",
+                (long long)search_ws_bytes, (long long)need);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool tp = plan->limiter.true_peak != 0;
+    std::vector<AlbumSearchTrack> album((size_t)tracks);
+    for (int k = 0; k < tracks; ++k) {
+        const Workspace ws = carve_workspace(*plan, layouts[k], t[k].d_workspace);
+        const float2* res = (const float2*)t[k].d_result_lr;
+        const int64_t n = layouts[k].target_frames;
+        mgb_track_state* state = t[k].d_state;
+        if (tp) {  // each track's detector once, as mgb_finalize_to_loudness runs it
+#ifdef MGB_EMULATE
+            memset(ws.tickets, 0, ws.limiter_zero_bytes);
+#else
+            if (cudaMemsetAsync(ws.tickets, 0, ws.limiter_zero_bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+            MGB_TRY(launch_true_peak_detect(plan->limiter.true_peak, res, n, ws.tp_plane, ws.tp_peak, st));
+        }
+        MGB_TRY(launch_scale(res, (float2*)d_out_limited[k], n, &state->gain, nullptr, st));
+        AlbumSearchTrack& e = album[k];
+        e.in = res;
+        e.s_metered = e.out = (float2*)d_out_limited[k];
+        e.frames = n;
+        e.gain = &state->gain;
+        e.peak_d = tp ? nullptr : &state->result_peak;
+        e.peak_bits = tp ? ws.tp_peak : nullptr;
+        e.zero = ws.tickets;
+        e.zero_bytes = ws.limiter_zero_bytes;
+        e.lookback = ws.lookback;
+        e.planes = ws.limiter_planes;
+        e.tp_d = tp ? ws.tp_plane : nullptr;
+    }
+    return run_album_loudness_search(plan->limiter, *meter, *target, album.data(), tracks, plan->d_limiter_tables,
+                                     d_search_ws, d_report, st);
+}
+
 // standalone limiter workspace: [0,4): peak bits  [16,20): ticket  [32,36): the true-peak detector's maximum  [256, kLimitHeader):
 // pole tables  [kLimitHeader, ...): look-back words, then the wide-window path's planes (none for the halo kernel), then the
 // true-peak detector's plane (true-peak mode only)

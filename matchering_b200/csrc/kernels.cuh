@@ -212,6 +212,25 @@ int run_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params&
                         const double* peak_d, const float* peak_bits, void* zero, int64_t zero_bytes, int* ticket,
                         void* lookback, void* planes, const void* tables, const float* tp_d, void* search_ws,
                         mgb_loudness_target_report* report, cudaStream_t stream);
+// album loudness targets: one entry per track, in album order (run_loudness_search's per-track arguments)
+struct AlbumSearchTrack {
+    const float2* in;         // the limiter's input (s / gain)
+    const float2* s_metered;  // s as samples, for the first meter run (the track's output buffer)
+    float2* out;
+    int64_t frames;
+    const double* gain;
+    const double* peak_d;
+    const float* peak_bits;
+    void* zero;  // the limiter's look-back words and ticket, cleared before every pass
+    int64_t zero_bytes;
+    void* lookback;
+    void* planes;
+    const float* tp_d;
+};
+int64_t album_loudness_target_search_bytes(const mgb_loudness_params& meter, int tracks, const int64_t* frames);
+int run_album_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& target,
+                              const AlbumSearchTrack* tracks, int count, const void* tables, void* search_ws,
+                              mgb_loudness_target_report* report, cudaStream_t stream);
 
 // fft test entry (api.cu) uses these -------------------------------------------------------------
 int launch_test_fft(int n, int is_f64, int dir, const void* in, void* out, int batch, const void* tw,

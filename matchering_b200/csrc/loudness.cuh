@@ -69,6 +69,68 @@ MeterWorkspace carve_meter(const mgb_loudness_params& lp, int64_t frames, void* 
     return w;
 }
 
+// The meter workspaces of an album's tracks carved from one block (mgb_album_loudness, the album loudness search):
+// every track's look-back words in one range (one clear), its own chunk shares and energies, and its momentary,
+// short-term and per-chunk peak arrays as consecutive slices of three pooled arrays.  A finish or integrated kernel
+// run once over a pooled array then meters the union of the tracks' windows, and no window straddles two tracks.
+// `all` describes the pooled arrays (chunks, nm and ns the sums; words and words_bytes the whole range); st_copy is
+// room for a copy of the pooled short-term array, which the finish kernel rewrites in place.
+struct AlbumMeter {
+    MeterWorkspace all;
+    double* st_copy;
+    int64_t total;
+};
+
+AlbumMeter carve_album_meter(const mgb_loudness_params& lp, int tracks, const int64_t* frames, void* base,
+                             MeterWorkspace* per_track) {
+    AlbumMeter a;
+    MeterWorkspace& all = a.all;
+    all.chunks = all.nb = all.nm = all.ns = 0;
+    int64_t words_bytes = 0;
+    for (int t = 0; t < tracks; ++t) {
+        const MeterWorkspace c = carve_meter(lp, frames[t], nullptr);
+        per_track[t] = c;
+        words_bytes += c.words_bytes;
+        all.chunks += c.chunks;
+        all.nb += c.nb;
+        all.nm += c.nm;
+        all.ns += c.ns;
+    }
+    unsigned char* p = (unsigned char*)base;
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) {
+        unsigned char* r = p ? p + off : nullptr;
+        off += align256(bytes);
+        return r;
+    };
+    all.words_bytes = words_bytes;
+    all.words = (LookbackWord*)take(words_bytes);
+    all.part = nullptr;
+    all.energy = nullptr;
+    all.peak = (double*)take(all.chunks * 4 * 8);
+    all.mom = (double*)take(all.nm * 8);
+    all.st = (double*)take(all.ns * 8);
+    a.st_copy = (double*)take(all.ns * 8);
+    int64_t words = 0, chunks = 0, nm = 0, ns = 0;
+    for (int t = 0; t < tracks; ++t) {
+        MeterWorkspace& w = per_track[t];
+        w.part = (double*)take(w.chunks * kMeterSlots * 8);
+        w.energy = (double*)take(w.nb * 8);
+        if (p) {
+            w.words = (LookbackWord*)((unsigned char*)all.words + words);
+            w.peak = all.peak + chunks * 4;
+            w.mom = all.mom + nm;
+            w.st = all.st + ns;
+        }
+        words += w.words_bytes;
+        chunks += w.chunks;
+        nm += w.nm;
+        ns += w.ns;
+    }
+    all.total = a.total = off;
+    return a;
+}
+
 __device__ __forceinline__ double warp_max_d(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -506,6 +568,34 @@ int loudness_validate(const mgb_loudness_params* lp) {
     return MGB_OK;
 }
 
+// The meter's kernels up to the finish for one track (its look-back words cleared by the caller)
+int launch_meter_windows(const mgb_loudness_params& lp, const float2* x, int64_t frames, const MeterWorkspace& w,
+                         cudaStream_t st) {
+    const MeterTables* tabs = (const MeterTables*)lp.d_tables;
+    const dim3 grid((unsigned)w.chunks);
+    const int* no_skip = nullptr;
+    if (lp.oversample == 4)
+        MGB_TRY(launch("loudness_kernel", loudness_kernel<4>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
+                       w.part, w.peak, tabs, no_skip));
+    else if (lp.oversample == 2)
+        MGB_TRY(launch("loudness_kernel", loudness_kernel<2>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
+                       w.part, w.peak, tabs, no_skip));
+    else
+        MGB_TRY(launch("loudness_kernel", loudness_kernel<1>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
+                       w.part, w.peak, tabs, no_skip));
+    const long long B = lp.block;
+    MGB_TRY(launch("loudness_fold_kernel", loudness_fold_kernel<>, dim3((unsigned)((w.nb + 255) / 256)), dim3(256), 0, st, B,
+                   (long long)w.nb, (const double*)w.part, w.energy, no_skip));
+    return launch("loudness_windows_kernel", loudness_windows_kernel<>, dim3((unsigned)((w.nm + 255) / 256)), dim3(256), 0,
+                  st, B, (long long)w.nb, (const double*)w.energy, w.mom, w.st, no_skip);
+}
+
+int launch_meter_finish(const MeterWorkspace& w, double* st_values, mgb_loudness_result* out, cudaStream_t st) {
+    return launch("loudness_finish_kernel", loudness_finish_kernel, dim3(1), dim3(kMeterFinishThreads), 0, st,
+                  (long long)w.chunks, (long long)w.nm, (long long)w.ns, (const double*)w.peak, (const double*)w.mom,
+                  st_values, out);
+}
+
 }  // namespace
 
 }  // namespace mgb
@@ -555,28 +645,57 @@ int mgb_loudness(const mgb_loudness_params* params, const float* d_lr, int64_t f
 #else
     if (cudaMemsetAsync(w.words, 0, w.words_bytes, st) != cudaSuccess) return cuda_status("memset");
 #endif
-    const mgb_loudness_params& lp = *params;
-    const float2* x = (const float2*)d_lr;
-    const MeterTables* tabs = (const MeterTables*)params->d_tables;
-    const dim3 grid((unsigned)w.chunks);
-    const int* no_skip = nullptr;
-    if (lp.oversample == 4)
-        MGB_TRY(launch("loudness_kernel", loudness_kernel<4>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs, no_skip));
-    else if (lp.oversample == 2)
-        MGB_TRY(launch("loudness_kernel", loudness_kernel<2>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs, no_skip));
-    else
-        MGB_TRY(launch("loudness_kernel", loudness_kernel<1>, grid, dim3(NT), 0, st, lp, x, (long long)frames, w.words,
-                       w.part, w.peak, tabs, no_skip));
-    const long long B = lp.block;
-    MGB_TRY(launch("loudness_fold_kernel", loudness_fold_kernel<>, dim3((unsigned)((w.nb + 255) / 256)), dim3(256), 0, st, B,
-                   (long long)w.nb, (const double*)w.part, w.energy, no_skip));
-    MGB_TRY(launch("loudness_windows_kernel", loudness_windows_kernel<>, dim3((unsigned)((w.nm + 255) / 256)), dim3(256), 0, st,
-                   B, (long long)w.nb, (const double*)w.energy, w.mom, w.st, no_skip));
-    return launch("loudness_finish_kernel", loudness_finish_kernel, dim3(1), dim3(kMeterFinishThreads), 0, st,
-                  (long long)w.chunks, (long long)w.nm, (long long)w.ns, (const double*)w.peak, (const double*)w.mom, w.st,
-                  d_result);
+    MGB_TRY(launch_meter_windows(*params, (const float2*)d_lr, frames, w, st));
+    return launch_meter_finish(w, w.st, d_result, st);
+}
+
+int64_t mgb_album_loudness_workspace_bytes(const mgb_loudness_params* params, int32_t tracks, const int64_t* frames) {
+    if (mgb::loudness_validate(params) != MGB_OK || tracks < 1 || tracks > MGB_MAX_ALBUM_TRACKS || frames == nullptr) return -1;
+    for (int t = 0; t < tracks; ++t)
+        if (frames[t] <= 0) return -1;
+    mgb::MeterWorkspace per_track[MGB_MAX_ALBUM_TRACKS];
+    return mgb::carve_album_meter(*params, tracks, frames, nullptr, per_track).total;
+}
+
+int mgb_album_loudness(const mgb_loudness_params* params, int32_t tracks, const float* const* d_lr, const int64_t* frames,
+                       void* d_workspace, int64_t workspace_bytes, mgb_loudness_result* d_album_result,
+                       mgb_loudness_result* d_track_results, void* stream) {
+    using namespace mgb;
+    MGB_TRY(loudness_validate(params));
+    MGB_REQUIRE(tracks >= 1 && tracks <= MGB_MAX_ALBUM_TRACKS, MGB_ERR_INVALID, "album loudness: %d tracks (1 .. %d)",
+                (int)tracks, MGB_MAX_ALBUM_TRACKS);
+    MGB_REQUIRE(d_lr != nullptr && frames != nullptr, MGB_ERR_INVALID, "album loudness: the track arrays are NULL");
+    auto aligned = [](const void* p) { return p != nullptr && ((uintptr_t)p & 15) == 0; };
+    for (int t = 0; t < tracks; ++t) {
+        MGB_REQUIRE(frames[t] > 0, MGB_ERR_INVALID, "album loudness: track %d has no frames", t);
+        MGB_REQUIRE(frames[t] <= (int64_t)INT32_MAX * LC, MGB_ERR_INVALID, "album loudness: track %d has too many frames", t);
+        MGB_REQUIRE(aligned(d_lr[t]), MGB_ERR_INVALID, "album loudness: track %d: NULL or misaligned samples", t);
+    }
+    MGB_REQUIRE(aligned(d_workspace) && aligned(d_album_result) && aligned(params->d_tables) &&
+                    (d_track_results == nullptr || aligned(d_track_results)),
+                MGB_ERR_INVALID, "album loudness: NULL or misaligned pointer (16 bytes needed)");
+    MeterWorkspace w[MGB_MAX_ALBUM_TRACKS];
+    const AlbumMeter a = carve_album_meter(*params, tracks, frames, d_workspace, w);
+    MGB_REQUIRE(workspace_bytes >= a.total, MGB_ERR_WORKSPACE, "album loudness: workspace of %lld bytes, need %lld",
+                (long long)workspace_bytes, (long long)a.total);
+    MGB_REQUIRE(a.all.ns <= INT32_MAX, MGB_ERR_INVALID, "album loudness: too many short-term windows");
+    cudaStream_t st = (cudaStream_t)stream;
+#ifdef MGB_EMULATE
+    memset(a.all.words, 0, a.all.words_bytes);
+#else
+    if (cudaMemsetAsync(a.all.words, 0, a.all.words_bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+    for (int t = 0; t < tracks; ++t) MGB_TRY(launch_meter_windows(*params, (const float2*)d_lr[t], frames[t], w[t], st));
+    if (d_track_results == nullptr) return launch_meter_finish(a.all, a.all.st, d_album_result, st);
+    // each track's finish gates its own slice of the short-term values in place: the album's reads a copy
+#ifdef MGB_EMULATE
+    memcpy(a.st_copy, a.all.st, a.all.ns * 8);
+#else
+    if (a.all.ns > 0 && cudaMemcpyAsync(a.st_copy, a.all.st, a.all.ns * 8, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+        return cuda_status("album loudness: short-term copy");
+#endif
+    for (int t = 0; t < tracks; ++t) MGB_TRY(launch_meter_finish(w[t], w[t].st, d_track_results + t, st));
+    return launch_meter_finish(a.all, a.st_copy, d_album_result, st);
 }
 
 }  // extern "C"

@@ -118,13 +118,19 @@ __global__ void loudness_target_step_kernel(mgb_loudness_target t, double thresh
     *out = *r;
 }
 
-int launch_pass_meter(const mgb_loudness_params& lp, const float2* x, int64_t frames, const MeterWorkspace& w,
-                      const int* skip, double* integrated, cudaStream_t st) {
+int clear_meter_words(const MeterWorkspace& w, cudaStream_t st) {
 #ifdef MGB_EMULATE
+    (void)st;
     memset(w.words, 0, w.words_bytes);
 #else
     if (cudaMemsetAsync(w.words, 0, w.words_bytes, st) != cudaSuccess) return cuda_status("memset");
 #endif
+    return MGB_OK;
+}
+
+// a pass's meter kernels up to the momentary windows, for one track (its look-back words cleared by the caller)
+int launch_pass_windows(const mgb_loudness_params& lp, const float2* x, int64_t frames, const MeterWorkspace& w,
+                        const int* skip, cudaStream_t st) {
     // the K-weighting does not depend on the oversampling; OS = 1 keeps the (unused) true peak cheap
     const MeterTables* tabs = (const MeterTables*)lp.d_tables;
     MGB_TRY(launch("loudness_kernel", loudness_kernel<1, true>, dim3((unsigned)w.chunks), dim3(NT), 0, st, lp, x,
@@ -132,10 +138,65 @@ int launch_pass_meter(const mgb_loudness_params& lp, const float2* x, int64_t fr
     const long long B = lp.block;
     MGB_TRY(launch("loudness_fold_kernel", loudness_fold_kernel<true>, dim3((unsigned)((w.nb + 255) / 256)), dim3(256), 0, st,
                    B, (long long)w.nb, (const double*)w.part, w.energy, skip));
-    MGB_TRY(launch("loudness_windows_kernel", loudness_windows_kernel<true>, dim3((unsigned)((w.nm + 255) / 256)), dim3(256),
-                   0, st, B, (long long)w.nb, (const double*)w.energy, w.mom, w.st, skip));
+    return launch("loudness_windows_kernel", loudness_windows_kernel<true>, dim3((unsigned)((w.nm + 255) / 256)), dim3(256),
+                  0, st, B, (long long)w.nb, (const double*)w.energy, w.mom, w.st, skip);
+}
+
+int launch_pass_integrated(const MeterWorkspace& w, const int* skip, double* integrated, cudaStream_t st) {
     return launch("loudness_integrated_kernel", loudness_integrated_kernel, dim3(1), dim3(kMeterFinishThreads), 0, st,
                   (long long)w.nm, (const double*)w.mom, skip, integrated);
+}
+
+int launch_pass_meter(const mgb_loudness_params& lp, const float2* x, int64_t frames, const MeterWorkspace& w,
+                      const int* skip, double* integrated, cudaStream_t st) {
+    MGB_TRY(clear_meter_words(w, st));
+    MGB_TRY(launch_pass_windows(lp, x, frames, w, skip, st));
+    return launch_pass_integrated(w, skip, integrated, st);
+}
+
+// ---- album loudness targets (mgb_album_finalize_to_loudness; DESIGN.md section 4 "Album loudness") ----------------
+// One drive x for K limiters: the search above runs unchanged on the album's integrated loudness (the integrated
+// kernel over the tracks' pooled momentary windows, carve_album_meter), and album_target_fanout_kernel turns each drive
+// into every track's pre-gain and early-out flag.
+
+// What the fan-out reads per track: the correction gain and the peak of s, as loudness_target_init_kernel reads them
+struct AlbumTargetTrack {
+    const double* gain;
+    const double* peak_d;
+    const float* peak_bits;
+};
+struct AlbumTargetTable {
+    int count;
+    AlbumTargetTrack t[MGB_MAX_ALBUM_TRACKS];
+};
+
+// The album search's header: the single-track search state, then the limiters' per-track inputs and what they follow
+// from (read once, on the first fan-out: the true-peak maximum sits in the limiter words every pass clears)
+struct AlbumTargetSearch {
+    TargetSearch s;
+    double pre_gain[MGB_MAX_ALBUM_TRACKS];
+    int32_t engaged[MGB_MAX_ALBUM_TRACKS];
+    double gain[MGB_MAX_ALBUM_TRACKS];
+    double peak_s[MGB_MAX_ALBUM_TRACKS];
+};
+constexpr int64_t kAlbumTargetHeader = (sizeof(AlbumTargetSearch) + 255) / 256 * 256;
+
+// one thread per track: target_set_pass's pre-gain and early-out flag at the drive the search chose, from the track's
+// own gain and peak (taken as loudness_target_init_kernel takes them, on the fan-out after it: `first`)
+__global__ void album_target_fanout_kernel(const __grid_constant__ AlbumTargetTable tab, double threshold, int first,
+                                           AlbumTargetSearch* __restrict__ h) {
+    const int t = threadIdx.x;
+    if (t >= tab.count || h->s.skip) return;
+    if (first) {
+        const AlbumTargetTrack e = tab.t[t];
+        h->gain[t] = *e.gain;
+        h->peak_s[t] = e.peak_d ? *e.peak_d : (double)(*e.peak_bits) * h->gain[t];
+    }
+    const double k = pow(10.0, h->s.x / 20.0);
+    h->pre_gain[t] = h->gain[t] * k;
+    const double peak = h->peak_s[t] * k;
+    const double r = fmax(peak, threshold) / threshold;
+    h->engaged[t] = (fabs(r - 1.0) <= 1e-8 + 1e-5 * 1.0) ? 0 : 1;
 }
 
 }  // namespace
@@ -190,6 +251,69 @@ int run_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params&
     return MGB_OK;
 }
 
+int64_t album_loudness_target_search_bytes(const mgb_loudness_params& meter, int tracks, const int64_t* frames) {
+    MeterWorkspace w[MGB_MAX_ALBUM_TRACKS];
+    return kAlbumTargetHeader + carve_album_meter(meter, tracks, frames, nullptr, w).total;
+}
+
+// The album's search on `stream`: run_loudness_search with every pass limiting and metering each track, the meter
+// pooled over the album.  Arguments checked by the caller.
+int run_album_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& t,
+                              const AlbumSearchTrack* tracks, int count, const void* tables, void* search_ws,
+                              mgb_loudness_target_report* report, cudaStream_t st) {
+    AlbumTargetSearch* h = (AlbumTargetSearch*)search_ws;
+    TargetSearch* s = &h->s;
+    int64_t frames[MGB_MAX_ALBUM_TRACKS];
+    AlbumTargetTable tab;
+    memset(&tab, 0, sizeof(tab));
+    tab.count = count;
+    for (int k = 0; k < count; ++k) {
+        frames[k] = tracks[k].frames;
+        tab.t[k].gain = tracks[k].gain;
+        tab.t[k].peak_d = tracks[k].peak_d;
+        tab.t[k].peak_bits = tracks[k].peak_bits;
+    }
+    MeterWorkspace w[MGB_MAX_ALBUM_TRACKS];
+    const AlbumMeter a = carve_album_meter(meter, count, frames, (unsigned char*)search_ws + kAlbumTargetHeader, w);
+    auto clear = [&](void* p, int64_t bytes) -> int {
+#ifdef MGB_EMULATE
+        memset(p, 0, bytes);
+#else
+        if (cudaMemsetAsync(p, 0, bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+        return MGB_OK;
+    };
+    auto pass_meter = [&](bool limited) -> int {
+        MGB_TRY(clear_meter_words(a.all, st));
+        for (int k = 0; k < count; ++k)
+            MGB_TRY(launch_pass_windows(meter, limited ? tracks[k].out : tracks[k].s_metered, frames[k], w[k], &s->skip, st));
+        return launch_pass_integrated(a.all, &s->skip, &s->measured, st);
+    };
+    auto fanout = [&](int first) {
+        return launch("album_target_fanout_kernel", album_target_fanout_kernel, dim3(1), dim3(count), 0, st, tab,
+                      lp.threshold, first, h);
+    };
+    MGB_TRY(clear(h, kAlbumTargetHeader));  // skip = 0 for the first meter run
+    MGB_TRY(pass_meter(false));
+    // (the init kernel's own pre-gain and flag are track 0's; the fan-out writes every track's)
+    MGB_TRY(launch("loudness_target_init_kernel", loudness_target_init_kernel, dim3(1), dim3(1), 0, st, t, lp.threshold,
+                   tracks[0].gain, tracks[0].peak_d, tracks[0].peak_bits, s));
+    MGB_TRY(fanout(1));
+    for (int pass = 1; pass <= MGB_LOUDNESS_TARGET_MAX_PASSES; ++pass) {
+        for (int k = 0; k < count; ++k) {
+            const AlbumSearchTrack& e = tracks[k];
+            MGB_TRY(clear(e.zero, e.zero_bytes));
+            MGB_TRY(launch_limiter(lp, e.in, e.out, e.frames, &h->pre_gain[k], nullptr, &h->engaged[k], (int*)e.zero,
+                                   e.lookback, e.planes, tables, st, false, e.tp_d, &s->skip));
+        }
+        MGB_TRY(pass_meter(true));
+        MGB_TRY(launch("loudness_target_step_kernel", loudness_target_step_kernel, dim3(1), dim3(1), 0, st, t, lp.threshold,
+                       pass, s, report));
+        if (pass < MGB_LOUDNESS_TARGET_MAX_PASSES) MGB_TRY(fanout(0));
+    }
+    return MGB_OK;
+}
+
 }  // namespace mgb
 
 extern "C" {
@@ -197,6 +321,17 @@ extern "C" {
 int64_t mgb_loudness_target_workspace_bytes(const mgb_loudness_params* meter, int64_t frames) {
     if (mgb::loudness_validate(meter) != MGB_OK || frames <= 0) return -1;
     return mgb::loudness_target_search_bytes(*meter, frames);
+}
+
+int64_t mgb_album_loudness_target_workspace_bytes(const mgb_loudness_params* meter, int32_t tracks,
+                                                  const mgb_track_layout* layouts) {
+    if (mgb::loudness_validate(meter) != MGB_OK || tracks < 1 || tracks > MGB_MAX_ALBUM_TRACKS || layouts == nullptr) return -1;
+    int64_t frames[MGB_MAX_ALBUM_TRACKS];
+    for (int t = 0; t < tracks; ++t) {
+        if (layouts[t].target_frames <= 0) return -1;
+        frames[t] = layouts[t].target_frames;
+    }
+    return mgb::album_loudness_target_search_bytes(*meter, tracks, frames);
 }
 
 // workspace: mgb_limit's (limit_impl's layout), then the search's

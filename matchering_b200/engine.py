@@ -265,6 +265,35 @@ def album_match(sessions: list, targets: list, d_profile: torch.Tensor, fir_out:
         album_ws.data_ptr(), ws_bytes, _stream_ptr(plan.device)))
 
 
+def album_finalize_to_loudness(sessions: list, target_lufs: float, need_no_limiter: bool = False,
+                               need_no_limiter_normalized: bool = False):
+    """Stage 4 of an album after album_match, with ONE limiter drive for every track searched until the album reads
+    `target_lufs` (mgb_album_finalize_to_loudness); the other two outputs as mgb_finalize writes them.
+    -> ([(limited, plain, normalized) per track], the album's device report)"""
+    from .loudness import device_meter, target_params
+    plan = sessions[0].plan
+    n = len(sessions)
+    outs = [s.finalize(False, need_no_limiter, need_no_limiter_normalized) for s in sessions]
+    limited = [torch.empty((int(s.layout.target_frames), 2), dtype=torch.float32, device=plan.device) for s in sessions]
+    table = (_native.AlbumTrack * n)()
+    for entry, session in zip(table, sessions):
+        entry.layout = C.pointer(session.layout)
+        entry.d_target_lr, entry.d_result_lr = None, session.result.data_ptr()
+        entry.d_workspace, entry.d_state = session.workspace.data_ptr(), session.state.data_ptr()
+    out_ptrs = (C.c_void_p * n)(*(t.data_ptr() for t in limited))
+    layouts = (_native.TrackLayout * n)(*(s.layout for s in sessions))
+    meter = device_meter(plan.tables.sample_rate, plan.device)
+    search_bytes = int(plan.lib.mgb_album_loudness_target_workspace_bytes(C.byref(meter.params), n, layouts))
+    if search_bytes < 0:
+        raise ValueError(plan.lib.mgb_last_error_string().decode("utf-8", "replace"))
+    search = torch.empty(search_bytes, dtype=torch.uint8, device=plan.device)
+    report = torch.empty(C.sizeof(_native.LoudnessTargetReport), dtype=torch.uint8, device=plan.device)
+    _native.check(plan.lib, plan.lib.mgb_album_finalize_to_loudness(
+        C.byref(plan.struct), n, table, out_ptrs, C.byref(meter.params), C.byref(target_params(target_lufs)),
+        search.data_ptr(), search_bytes, report.data_ptr(), _stream_ptr(plan.device)))
+    return [(lim, plain, normalized) for lim, (_, plain, normalized) in zip(limited, outs)], report
+
+
 # ------------------------------------------------------------------------------------------------
 # host arrays in, host arrays out (the reference's seam: pageable float64 numpy, core.py:77-86)
 # ------------------------------------------------------------------------------------------------

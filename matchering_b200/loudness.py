@@ -114,6 +114,34 @@ class DeviceMeter:
             raw = out.cpu().numpy().tobytes()
         return Loudness.from_result(_native.LoudnessResult.from_buffer_copy(raw))
 
+    def measure_album(self, xs: list) -> "AlbumLoudness":
+        """xs: (N_t, 2) float32 CUDA tensors on this meter's device, one per track (mgb_album_loudness)."""
+        import torch
+        from .engine import _stream_ptr
+        n = len(xs)
+        frames = (C.c_int64 * n)(*(int(x.shape[0]) for x in xs))
+        ptrs = (C.c_void_p * n)(*(x.data_ptr() for x in xs))
+        ws_bytes = int(self.lib.mgb_album_loudness_workspace_bytes(C.byref(self.params), n, frames))
+        size = C.sizeof(_native.LoudnessResult)
+        with torch.cuda.device(self.device):
+            ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=self.device)
+            out = torch.empty((n + 1) * size, dtype=torch.uint8, device=self.device)  # the album, then each track
+            _native.check(self.lib, self.lib.mgb_album_loudness(C.byref(self.params), n, ptrs, frames, ws.data_ptr(),
+                                                               ws_bytes, out.data_ptr(), out.data_ptr() + size,
+                                                               _stream_ptr(self.device)))
+            raw = out.cpu().numpy().tobytes()
+        results = [Loudness.from_result(_native.LoudnessResult.from_buffer_copy(raw[k * size:(k + 1) * size]))
+                   for k in range(n + 1)]
+        return AlbumLoudness(results[0], tuple(results[1:]))
+
+
+@dataclass(frozen=True)
+class AlbumLoudness:
+    """An album's meter (mg.album_loudness): `album` meters the tracks as one programme (the gates and the loudness
+    range over the union of every track's windows, the maxima over the tracks), `tracks` each track on its own."""
+    album: Loudness
+    tracks: tuple
+
 
 _METERS: dict = {}
 
@@ -167,3 +195,57 @@ def loudness(audio, sample_rate: int | None = None) -> Loudness:
     meter = device_meter(sample_rate)
     from .engine import to_device_f32
     return meter.measure(to_device_f32(a, meter.device))
+
+
+def _album_audio(audio, sample_rate):
+    """One album track -> ((N, 2) float32 CUDA tensor or float numpy array, its rate or None)."""
+    import torch
+    if isinstance(audio, (str, bytes)) or hasattr(audio, "__fspath__"):
+        import os
+        from .loader import load
+        path = os.fsdecode(os.fspath(audio))
+        audio, rate = load(path, "target", os.path.dirname(os.path.abspath(path)))
+        if sample_rate is not None and int(sample_rate) != int(rate):
+            raise ValueError(f"album_loudness: '{path}' is at {rate} Hz, not {sample_rate}")
+        _check_shape(np.shape(audio))
+        return audio, int(rate)
+    if isinstance(audio, torch.Tensor):
+        _check_shape(audio.shape)
+        if not audio.is_cuda or audio.dtype != torch.float32:
+            raise ValueError("album_loudness: tensors must be float32 on a CUDA device (numpy arrays may be float64)")
+        return audio, None
+    a = np.asarray(audio)
+    _check_shape(a.shape)
+    if a.dtype not in (np.float32, np.float64):
+        raise ValueError(f"album_loudness: float32 or float64 samples, not {a.dtype}")
+    return a, None
+
+
+def album_loudness(tracks, sample_rate: int | None = None) -> AlbumLoudness:
+    """Meter an album as one programme: `tracks` is a list of file paths, (N, 2) numpy arrays or (N, 2) float32 CUDA
+    tensors, all at one rate (`sample_rate` is required unless every track is a file).  The album's integrated loudness
+    and loudness range gate the union of every track's 400 ms and 3 s windows, each window counting once and none
+    straddling two tracks (libebur128's ebur128_loudness_global_multiple); its maxima and peaks are the tracks' maxima.
+    -> AlbumLoudness(album, tracks), the second each track's own meter, as mg.loudness reads it."""
+    import torch
+    tracks = list(tracks)
+    if not tracks:
+        raise ValueError("album_loudness: an album needs at least one track")
+    if len(tracks) > _native.MGB_MAX_ALBUM_TRACKS:
+        raise ValueError(f"album_loudness: {len(tracks)} tracks, at most {_native.MGB_MAX_ALBUM_TRACKS}")
+    loaded = [_album_audio(t, sample_rate) for t in tracks]
+    rates = {r for _, r in loaded if r is not None}
+    if sample_rate is not None:
+        rates.add(int(sample_rate))
+    if len(rates) > 1:
+        raise ValueError(f"album_loudness: the tracks are at different rates {sorted(rates)}")
+    if not rates:
+        raise ValueError("album_loudness: sample_rate is required for arrays and tensors")
+    rate = rates.pop()
+    devices = {a.device for a, _ in loaded if isinstance(a, torch.Tensor)}
+    if len(devices) > 1:
+        raise ValueError("album_loudness: the tensors are on different devices")
+    meter = device_meter(rate, devices.pop() if devices else None)
+    from .engine import to_device_f32
+    xs = [a.contiguous() if isinstance(a, torch.Tensor) else to_device_f32(a, meter.device) for a, _ in loaded]
+    return meter.measure_album(xs)

@@ -3,11 +3,13 @@ same four stages and the same info codes between them; every array operation run
 libmatchering_b200 on the current CUDA device."""
 from __future__ import annotations
 
+import math
+
 import torch
 
 from . import _native, plan as _plan
 from .defaults import Config
-from .engine import (TrackSession, album_match, get_native_plan, get_plan, host_array_ok, stages_main_host,
+from .engine import (TrackSession, album_finalize_to_loudness, album_match, get_native_plan, get_plan, host_array_ok, stages_main_host,
                      stages_main_host_profiled, to_device_f32, to_host_like)
 from .log import Code, info, debug, debug_line, debug_enabled
 from .profile import ReferenceProfile
@@ -218,35 +220,45 @@ def main_native_device(target, sample_rate: int, reference, config: Config, need
 
 
 def main_album(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
-               need_no_limiter_normalized: bool = False):
+               need_no_limiter_normalized: bool = False, album_loudness_target: float | None = None):
     """Master the K tracks of an album against one reference with ONE level match and ONE matching FIR, from
     statistics pooled over every piece of every track (DESIGN.md section 4 "Album mastering"), so the tracks keep their
     relative levels and share one tonal correction.  targets: a list of (N_t, 2) stereo arrays at
     config.internal_sample_rate, numpy or torch; reference: samples or a ReferenceProfile.  Returns one
     (result, result_no_limiter, result_no_limiter_normalized) per track, None where not requested, in each target's
     array type.  The normalized result is normalised per track, as in `main`.  A one-track album is `main` with the
-    reference's profile, bit for bit."""
-    outs = main_album_device(targets, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
+    reference's profile, bit for bit.
+
+    album_loudness_target (LUFS): drive every track's limiter with ONE gain, searched until the album, metered as one
+    programme (mg.album_loudness), reads that integrated loudness (DESIGN.md section 4 "Album loudness").  Where no
+    limiter engages every track gets the same gain, so the relative levels hold exactly.  Only the limited results
+    are targeted."""
+    outs = main_album_device(targets, reference, config, need_default, need_no_limiter, need_no_limiter_normalized,
+                             album_loudness_target=album_loudness_target)
     return [tuple(None if t is None else to_host_like(t, target) for t in track) for track, target in zip(outs, targets)]
 
 
-def album_check(count: int, config: Config) -> None:
+def album_check(count: int, config: Config, album_loudness_target=None) -> None:
     """The album requests main_album refuses before any device work."""
+    if album_loudness_target is not None and not (
+            isinstance(album_loudness_target, (int, float)) and not isinstance(album_loudness_target, bool)
+            and math.isfinite(album_loudness_target) and -70 < album_loudness_target < 0):
+        raise ValueError("album_loudness_target must be None or a finite LUFS value in (-70, 0)")
     if count < 1:
         raise ValueError("an album needs at least one track")
     if count > _native.MGB_MAX_ALBUM_TRACKS:
         raise ValueError(f"an album of {count} tracks: at most {_native.MGB_MAX_ALBUM_TRACKS} are mastered together")
     if config.loudness_target is not None:
         raise ValueError("Config(loudness_target=...) is not available for albums: a target per track would undo the "
-                         "album's level relation")
+                         "album's level relation; album_loudness_target=... drives the whole album with one gain")
 
 
 def main_album_device(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
-                      need_no_limiter_normalized: bool = False, fir_out=None):
+                      need_no_limiter_normalized: bool = False, fir_out=None, album_loudness_target: float | None = None):
     """`main_album` with the results left on the device as float32 CUDA tensors.  fir_out: optional (2, fft_size)
     float64 CUDA tensor that receives the album's mid and side FIRs."""
     targets = list(targets)
-    album_check(len(targets), config)
+    album_check(len(targets), config, album_loudness_target)
     for target in targets:
         if target.ndim != 2 or target.shape[1] != 2:
             raise ValueError("every target must be a (frames, 2) stereo array")
@@ -272,11 +284,21 @@ def main_album_device(targets, reference, config: Config, need_default: bool = T
 
         debug_line()
         info(Code.INFO_FINALIZING)
-        outs = [s.finalize(need_default, need_no_limiter, need_no_limiter_normalized) for s in sessions]
+        report = None
+        if need_default and album_loudness_target is not None:
+            outs, report = album_finalize_to_loudness(sessions, float(album_loudness_target), need_no_limiter,
+                                                      need_no_limiter_normalized)
+        else:
+            outs = [s.finalize(need_default, need_no_limiter, need_no_limiter_normalized) for s in sessions]
         if debug_enabled():
             st = sessions[0].read_state()
             debug(f"The album's {st.target_loud_pieces} loud pieces of {sum(int(s.layout.target_divisions) for s in sessions)}"
                   f" give one RMS coefficient: {to_db(st.rms_coefficient)}")
             for step in range(st.steps_done):
                 debug(f"Album RMS correction #{step + 1}: {to_db(st.correction[step])}")
+            if report is not None:
+                from .loudness import LoudnessTarget, debug_target
+                raw = report.cpu().numpy().tobytes()
+                debug_target(LoudnessTarget.from_report(float(album_loudness_target),
+                                                        _native.LoudnessTargetReport.from_buffer_copy(raw)))
     return outs
