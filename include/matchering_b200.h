@@ -484,6 +484,58 @@ int mgb_album_finalize_to_loudness(const mgb_plan* plan, int32_t tracks, const m
                                    const mgb_loudness_target* target, void* d_search_ws, int64_t search_ws_bytes,
                                    mgb_loudness_target_report* d_report, void* stream);
 
+/* ---- linked versions: a mix's instrumental, a cappella, TV mix or clean edit mastered with the main's match and its
+ * limiter gain, so that every version nulls against the master (DESIGN.md section 4 "Linked versions") --------------
+ * The main x_0 runs stages 1-3 as a single job (paired or profiled).  Each version x_v (the same frame count) is then
+ * convolved with the main's FIR spectra (c0 folded in) and scaled by the main's correction gain G; no correction step
+ * runs on it.  Stage 4 limits all of them with ONE gain envelope e, computed from D[n] = the maximum over the main and
+ * every version of the limiter's detector (max(|L|, |R|), or the true-peak detector d[n]) of s_v = result_v * G:
+ *   limited_v    = s_v * e * final_amplitude_coefficient   (the same float64 gain for every entry)
+ *   no limiter   = s_v
+ *   normalized_v = s_v / max(eps, G * max(D) / threshold)
+ * Where no version's detector exceeds the main's, the main's outputs are the single job's bit for bit. */
+#define MGB_MAX_VERSIONS 8
+typedef struct mgb_version_track {
+    const mgb_track_layout* layout; /* mgb_track_layout_init_profiled of the plan, for the main's frame count */
+    const float* d_target_lr;       /* the version: layout->target_frames stereo frames at the plan's rate */
+    float* d_result_lr;             /* its stage-2 result (neither a target nor another result) */
+    void* d_workspace;              /* layout->workspace_bytes, its own */
+    mgb_track_state* d_state;       /* its own; starts as a copy of the main's */
+} mgb_version_track;
+/* Stage 2 of `versions` versions (1 .. MGB_MAX_VERSIONS) with the main's FIR, after the main's mgb_correct_levels
+ * (plan, layout, d_workspace and d_state are the main's).  A version takes the float64 convolution where the main does or
+ * where the main's rule, applied to the version's own peak, calls for it.  MGB_ERR_INVALID: a bad count, NULL or
+ * misaligned pointers, a frame count that is not the main's, a layout that is not this plan's profiled layout of it, a
+ * result that is any target or result. */
+int mgb_version_match_frequencies(const mgb_plan* plan, const mgb_track_layout* layout, const void* d_workspace,
+                                  const mgb_track_state* d_state, int32_t versions, const mgb_version_track* v, void* stream);
+/* One entry of stage 4: entry 0 is the main (its d_result_lr from mgb_match_frequencies), then the versions' results.
+ * Each output may be NULL, as in mgb_finalize. */
+typedef struct mgb_version_entry {
+    const float* d_result_lr;
+    float* d_out_limited;
+    float* d_out_no_limiter;
+    float* d_out_normalized;
+} mgb_version_entry;
+/* device scratch of stage 4 with versions (the linked detector plane, its maximum, a copy of the main's scalars); -1 for
+ * bad arguments */
+int64_t mgb_versions_workspace_bytes(const mgb_plan* plan, const mgb_track_layout* layout);
+/* Stage 4 of the main and its versions: `entries` = 1 + versions (1 .. 1 + MGB_MAX_VERSIONS) entries, the main first;
+ * d_workspace and d_state are the main's.  d_state is not changed.  MGB_ERR_INVALID: a bad count, NULL or misaligned
+ * pointers, an output that aliases any result or another output; MGB_ERR_WORKSPACE: a short versions workspace. */
+int mgb_finalize_versions(const mgb_plan* plan, const mgb_track_layout* layout, int32_t entries, const mgb_version_entry* e,
+                          void* d_workspace, const mgb_track_state* d_state, void* d_versions_ws, int64_t versions_ws_bytes,
+                          void* stream);
+/* The limited outputs at a loudness target (mgb_finalize_to_loudness's search on the main's integrated loudness, its
+ * limiter reading D): every entry receives limit at the drive x* the search ends on, no final_amplitude_coefficient.
+ * Every entry's d_out_limited is required, and its other two outputs must be NULL (mgb_finalize_versions writes those).
+ * d_report (device): the main's report.  Errors as mgb_finalize_versions and mgb_finalize_to_loudness. */
+int mgb_finalize_versions_to_loudness(const mgb_plan* plan, const mgb_track_layout* layout, const mgb_loudness_params* meter,
+                                      const mgb_loudness_target* target, int32_t entries, const mgb_version_entry* e,
+                                      void* d_workspace, const mgb_track_state* d_state, void* d_versions_ws,
+                                      int64_t versions_ws_bytes, void* d_search_ws, int64_t search_ws_bytes,
+                                      mgb_loudness_target_report* d_report, void* stream);
+
 /* ---- whole job with HOST buffers (the call the end-to-end benchmark times) --------------------
  * h_* are host pointers (pinned for full speed).  Copies target and reference to the device,
  * runs stages 1-4 and copies the requested outputs back; synchronises `stream` before returning.

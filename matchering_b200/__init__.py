@@ -24,3 +24,8 @@ def process(*args, **kwargs):
 def process_album(*args, **kwargs):
     from .core import process_album as _process_album
     return _process_album(*args, **kwargs)
+
+
+def process_versions(*args, **kwargs):
+    from .core import process_versions as _process_versions
+    return _process_versions(*args, **kwargs)

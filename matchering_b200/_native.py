@@ -144,6 +144,25 @@ class AlbumTrack(C.Structure):
 MGB_MAX_ALBUM_TRACKS = 64
 
 
+class VersionTrack(C.Structure):
+    """mgb_version_track: one version of mgb_version_match_frequencies (device pointers)."""
+    _fields_ = [
+        ("layout", C.POINTER(TrackLayout)), ("d_target_lr", C.c_void_p), ("d_result_lr", C.c_void_p),
+        ("d_workspace", C.c_void_p), ("d_state", C.c_void_p),
+    ]
+
+
+class VersionEntry(C.Structure):
+    """mgb_version_entry: one entry of mgb_finalize_versions, the main first (device pointers, outputs optional)."""
+    _fields_ = [
+        ("d_result_lr", C.c_void_p), ("d_out_limited", C.c_void_p), ("d_out_no_limiter", C.c_void_p),
+        ("d_out_normalized", C.c_void_p),
+    ]
+
+
+MGB_MAX_VERSIONS = 8
+
+
 MGB_REFERENCE_PROFILE_VERSION = 1
 
 
@@ -250,6 +269,15 @@ PROTOTYPES = {
     "mgb_album_workspace_bytes": (C.c_int64, [C.POINTER(Plan), C.c_int32, C.POINTER(TrackLayout)]),
     "mgb_album_match": (C.c_int, [C.POINTER(Plan), C.c_int32, C.POINTER(AlbumTrack), C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.c_int64, C.c_void_p]),
+    "mgb_version_match_frequencies": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_int32,
+                                                C.POINTER(VersionTrack), C.c_void_p]),
+    "mgb_versions_workspace_bytes": (C.c_int64, [C.POINTER(Plan), C.POINTER(TrackLayout)]),
+    "mgb_finalize_versions": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_int32, C.POINTER(VersionEntry), C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mgb_finalize_versions_to_loudness": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.POINTER(LoudnessParams),
+                                                    C.POINTER(LoudnessTargetParams), C.c_int32, C.POINTER(VersionEntry),
+                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                                    C.c_void_p, C.c_void_p]),
     "mgb_correct_levels": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p]),
     "mgb_finalize": (C.c_int, [C.POINTER(Plan), C.POINTER(TrackLayout), C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -147,6 +147,72 @@ def process_album(targets: list, reference, results: list, config: Config = None
     info(Code.INFO_COMPLETED)
 
 
+def process_versions(targets: list, reference, results: list, config: Config = None):
+    """Master a mix and its versions as linked versions (stages.main_versions): `targets[0]` is the main mix's file,
+    the others its versions' (instrumental, a cappella, TV mix, clean edit), all of one length and one sample rate;
+    `results` holds a list of Result per target, as mg.process takes them.  Every file is loaded and checked as
+    mg.process loads its target.  The versions take the main's match and the main's limiter gain, so that every
+    master nulls against the main's: main master - instrumental master is the vocal through the same chain.
+    `reference` is a file path or a ReferenceProfile.  Versions of another length or rate, more than 8 versions and
+    native-rate targets off the internal rate are refused before any device work."""
+    from ._native import MGB_MAX_VERSIONS
+    from .stages import main_versions_device, versions_check
+    if config is None:
+        config = Config()
+    targets, results = list(targets), list(results)
+    if not targets or len(targets) != len(results):
+        raise ValueError(f"process_versions: {len(targets)} targets and {len(results)} result lists")
+    if len(targets) - 1 > MGB_MAX_VERSIONS:
+        raise ValueError(f"process_versions: {len(targets) - 1} versions, at most {MGB_MAX_VERSIONS}")
+    if any(not r for r in results):
+        raise ValueError("process_versions: every target needs at least one Result")
+    rates = [_file_rate(t) for t in targets]
+    if config.native_rate:
+        for t, rate in zip(targets, rates):
+            if rate is not None and rate != config.internal_sample_rate:
+                raise ValueError(f"process_versions: '{t}' is at {rate} Hz; versions are mastered at the internal rate "
+                                 f"({config.internal_sample_rate} Hz), not at native rates")
+    for t, rate in zip(targets[1:], rates[1:]):
+        if rate is not None and rates[0] is not None and rate != rates[0]:
+            raise ValueError(f"process_versions: '{t}' is at {rate} Hz, the main mix at {rates[0]} Hz")
+    debug_line()
+    info(Code.INFO_LOADING)
+    temp_folder = config.temp_folder if config.temp_folder else get_temp_folder([r for rs in results for r in rs])
+    reference_audio = None
+    if isinstance(reference, ReferenceProfile):
+        reference.check_config(config)
+    else:
+        reference_audio, reference_rate = _load_and_check(reference, "reference", temp_folder, config)
+        if (reference_rate != config.internal_sample_rate or reference_audio.shape[1] != 2
+                or not reference_audio.shape[0] > config.fft_size):
+            raise ModuleError(Code.ERROR_VALIDATION)
+    audios = []
+    for t in targets:
+        audio, rate, _, native_rate = _load_and_check_target(t, temp_folder, config)
+        if native_rate != config.internal_sample_rate:
+            raise ValueError(f"process_versions: '{t}' is at {native_rate} Hz; versions are mastered at the internal rate")
+        if reference_audio is not None and not config.allow_equality:
+            _check_equality_any(audio, reference_audio)
+        if rate != config.internal_sample_rate or audio.shape[1] != 2 or not audio.shape[0] > config.fft_size:
+            raise ModuleError(Code.ERROR_VALIDATION)
+        audios.append(audio)
+    versions_check(audios, config)
+
+    everything = [r for rs in results for r in rs]
+    needs = dict(need_default=any(r.use_limiter for r in everything),
+                 need_no_limiter=any(not r.use_limiter and not r.normalize for r in everything),
+                 need_no_limiter_normalized=any(not r.use_limiter and r.normalize for r in everything))
+    outs = main_versions_device(audios, reference if reference_audio is None else reference_audio, config, **needs)
+    debug_line()
+    info(Code.INFO_EXPORTING)
+    for (limited, plain, normalized), wanted_list in zip(outs, results):
+        for wanted in wanted_list:
+            audio = limited if wanted.use_limiter else (normalized if wanted.normalize else plain)
+            _export(wanted, audio, config.internal_sample_rate)
+    debug_line()
+    info(Code.INFO_COMPLETED)
+
+
 def _file_rate(path) -> int | None:
     """The sample rate a file's header states, or None when it cannot be read without decoding."""
     from . import wavio

@@ -845,6 +845,241 @@ int mgb_album_match(const mgb_plan* plan, int32_t tracks, const mgb_album_track*
     return launch_album_correction_final(*plan, album.data(), tracks, st);
 }
 
+// ---- linked versions ----------------------------------------------------------------------------------------------
+// Stage 4's scratch with versions: a copy of the main's scalars (whose normalisation coefficient and early-out flag the
+// linked detector's maximum replaces), that maximum, and the linked detector plane D.
+struct VersionRegions {
+    mgb_track_state* state;
+    float* d_max;
+    float* d;
+    int64_t total_bytes;
+};
+static VersionRegions carve_versions(const mgb_track_layout& L, void* base_ptr) {
+    VersionRegions r;
+    const uintptr_t base = reinterpret_cast<uintptr_t>(base_ptr);
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) {
+        unsigned char* p = reinterpret_cast<unsigned char*>(base + (uintptr_t)off);
+        off += align256(bytes);
+        return p;
+    };
+    r.state = (mgb_track_state*)take(sizeof(mgb_track_state));
+    r.d_max = (float*)take(4);
+    r.d = (float*)take(L.target_frames * 4);
+    r.total_bytes = off;
+    return r;
+}
+
+static int device_copy(void* dst, const void* src, size_t bytes, cudaStream_t st) {
+#ifdef MGB_EMULATE
+    (void)st;
+    memcpy(dst, src, bytes);
+#else
+    if (cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return cuda_status("versions: copy");
+#endif
+    return MGB_OK;
+}
+static int device_zero(void* dst, size_t bytes, cudaStream_t st) {
+#ifdef MGB_EMULATE
+    (void)st;
+    memset(dst, 0, bytes);
+#else
+    if (cudaMemsetAsync(dst, 0, bytes, st) != cudaSuccess) return cuda_status("versions: memset");
+#endif
+    return MGB_OK;
+}
+
+int64_t mgb_versions_workspace_bytes(const mgb_plan* plan, const mgb_track_layout* L) {
+    if (check_plan(plan) != MGB_OK || L == nullptr || L->target_frames <= plan->fft_size) return -1;
+    return carve_versions(*L, nullptr).total_bytes;
+}
+
+int mgb_version_match_frequencies(const mgb_plan* plan, const mgb_track_layout* L, const void* d_workspace,
+                                  const mgb_track_state* d_state, int32_t versions, const mgb_version_track* v, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_REQUIRE(versions >= 1 && versions <= MGB_MAX_VERSIONS, MGB_ERR_INVALID, "versions: %d versions (1 .. %d)", (int)versions,
+                MGB_MAX_VERSIONS);
+    MGB_REQUIRE(v != nullptr, MGB_ERR_INVALID, "versions: the version table is NULL");
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_state, "d_state"));
+    for (int k = 0; k < versions; ++k) {
+        const mgb_track_layout* VL = v[k].layout;
+        MGB_REQUIRE(VL != nullptr && VL->target_frames == L->target_frames, MGB_ERR_INVALID,
+                    "versions: version %d has no layout or not the main's %lld frames", k + 1, (long long)L->target_frames);
+        mgb_track_layout want;
+        if (mgb_track_layout_init_profiled(plan, VL->target_frames, &want) != MGB_OK || memcmp(&want, VL, sizeof(want)) != 0) {
+            set_error("versions: version %d: the layout is not this plan's profiled layout of %lld frames", k + 1,
+                      (long long)VL->target_frames);
+            return MGB_ERR_INVALID;
+        }
+        MGB_TRY(check_aligned(v[k].d_target_lr, "d_target_lr"));
+        MGB_TRY(check_aligned(v[k].d_result_lr, "d_result_lr"));
+        MGB_TRY(check_aligned(v[k].d_workspace, "d_workspace"));
+        MGB_TRY(check_aligned(v[k].d_state, "d_state"));
+        for (int j = 0; j < versions; ++j) {
+            MGB_REQUIRE((const void*)v[k].d_result_lr != (const void*)v[j].d_target_lr &&
+                            (j == k || (const void*)v[k].d_result_lr != (const void*)v[j].d_result_lr),
+                        MGB_ERR_INVALID, "versions: version %d's d_result_lr is a target or another result", k + 1);
+        }
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const Workspace mws = carve_workspace(*plan, *L, const_cast<void*>(d_workspace));
+    for (int k = 0; k < versions; ++k) {
+        Workspace ws = carve_workspace(*plan, *v[k].layout, v[k].d_workspace);
+        mgb_track_state* state = v[k].d_state;
+        // the main's scalars (c0 is in the FIR spectra; the FIR's peaks choose the precision), with what the convolution
+        // measures for itself cleared; the precision rule sees max(the main's peak, the version's own)
+        MGB_TRY(device_zero(ws.zero_begin, ws.zero_end - ws.zero_begin, st));
+        MGB_TRY(device_copy(state, d_state, sizeof(mgb_track_state), st));
+        MGB_TRY(device_zero(&state->conv_peak_bits, sizeof(float), st));
+        MGB_TRY(device_zero(&state->conv_precise, sizeof(int32_t), st));
+        MGB_TRY(device_copy(ws.target_peak, mws.target_peak, sizeof(float), st));
+        MGB_TRY(launch_absmax((const float2*)v[k].d_target_lr, v[k].layout->target_frames, ws.target_peak, st));
+        ws.h_mid = mws.h_mid;
+        ws.h_side = mws.h_side;
+        MGB_TRY(launch_convolve(*plan, *v[k].layout, (const float2*)v[k].d_target_lr, (float2*)v[k].d_result_lr, ws, state, st));
+    }
+    return MGB_OK;
+}
+
+// the entries' checks shared by both stage-4 calls; loudness: every limited output required, the other two NULL
+static int check_version_entries(int32_t entries, const mgb_version_entry* e, bool loudness) {
+    MGB_REQUIRE(entries >= 1 && entries <= 1 + MGB_MAX_VERSIONS, MGB_ERR_INVALID, "versions: %d entries (1 .. %d)", (int)entries,
+                1 + MGB_MAX_VERSIONS);
+    MGB_REQUIRE(e != nullptr, MGB_ERR_INVALID, "versions: the entry table is NULL");
+    for (int k = 0; k < entries; ++k) {
+        MGB_TRY(check_aligned(e[k].d_result_lr, "d_result_lr"));
+        const float* outs[3] = {e[k].d_out_limited, e[k].d_out_no_limiter, e[k].d_out_normalized};
+        if (loudness) {
+            MGB_TRY(check_aligned(outs[0], "d_out_limited"));
+            MGB_REQUIRE(!outs[1] && !outs[2], MGB_ERR_INVALID,
+                        "versions to loudness: entry %d: only d_out_limited is written here (the others must be NULL)", k);
+        }
+        for (int i = 0; i < 3; ++i) {
+            if (!outs[i]) continue;
+            MGB_TRY(check_aligned(outs[i], "output"));
+            for (int j = 0; j < entries; ++j) {
+                MGB_REQUIRE((const void*)outs[i] != (const void*)e[j].d_result_lr, MGB_ERR_INVALID,
+                            "versions: an output of entry %d is the result of entry %d", k, j);
+                const float* other[3] = {e[j].d_out_limited, e[j].d_out_no_limiter, e[j].d_out_normalized};
+                for (int m = 0; m < 3; ++m)
+                    MGB_REQUIRE((j == k && m == i) || outs[i] != other[m], MGB_ERR_INVALID,
+                                "versions: an output of entry %d is another output", k);
+            }
+        }
+    }
+    return MGB_OK;
+}
+
+// the linked detector over every entry's result into r.d / r.d_max (true-peak mode: the main's detector, then each
+// version's added to it)
+static int versions_detect(const mgb_plan& plan, int64_t n, int32_t entries, const mgb_version_entry* e, const VersionRegions& r,
+                           cudaStream_t st) {
+    MGB_TRY(device_zero(r.d_max, 4, st));
+    if (plan.limiter.true_peak) {
+        MGB_TRY(launch_true_peak_detect(plan.limiter.true_peak, (const float2*)e[0].d_result_lr, n, r.d, r.d_max, st));
+        for (int k = 1; k < entries; ++k)
+            MGB_TRY(launch_true_peak_accumulate(plan.limiter.true_peak, (const float2*)e[k].d_result_lr, n, r.d, r.d_max, st));
+        return MGB_OK;
+    }
+    VersionPlanes all;
+    memset(&all, 0, sizeof(all));
+    all.count = entries;
+    for (int k = 0; k < entries; ++k) all.in[k] = (const float2*)e[k].d_result_lr;
+    return launch_versions_detect(all, n, r.d, r.d_max, st);
+}
+
+int mgb_finalize_versions(const mgb_plan* plan, const mgb_track_layout* L, int32_t entries, const mgb_version_entry* e,
+                          void* d_workspace, const mgb_track_state* d_state, void* d_versions_ws, int64_t versions_ws_bytes,
+                          void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_TRY(check_version_entries(entries, e, false));
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_versions_ws, "d_versions_ws"));
+    const int64_t need = mgb_versions_workspace_bytes(plan, L);
+    MGB_REQUIRE(need > 0, MGB_ERR_INVALID, "versions: the layout has no more than fft_size frames");
+    MGB_REQUIRE(versions_ws_bytes >= need, MGB_ERR_WORKSPACE, "versions: workspace of %lld bytes, need %lld",
+                (long long)versions_ws_bytes, (long long)need);
+    cudaStream_t st = (cudaStream_t)stream;
+    const Workspace ws = carve_workspace(*plan, *L, d_workspace);
+    const VersionRegions r = carve_versions(*L, d_versions_ws);
+    const int64_t n = L->target_frames;
+    VersionPlanes lim;
+    memset(&lim, 0, sizeof(lim));
+    bool normalized = false;
+    for (int k = 0; k < entries; ++k) {
+        if (e[k].d_out_limited) {
+            lim.in[lim.count] = (const float2*)e[k].d_result_lr;
+            lim.out[lim.count++] = (float2*)e[k].d_out_limited;
+        }
+        normalized = normalized || e[k].d_out_normalized;
+    }
+    MGB_TRY(device_copy(r.state, d_state, sizeof(mgb_track_state), st));
+    if (lim.count || normalized) {
+        // max(D) in place of the main's own peak: the normalisation coefficient and the early-out (true_peak_final_kernel's
+        // rule is correction_final_kernel's, from any peak)
+        MGB_TRY(versions_detect(*plan, n, entries, e, r, st));
+        MGB_TRY(launch_true_peak_final(r.d_max, plan->min_value, plan->threshold, r.state, st));
+    }
+    for (int k = 0; k < entries; ++k) {
+        const float2* res = (const float2*)e[k].d_result_lr;
+        if (e[k].d_out_normalized)
+            MGB_TRY(launch_scale(res, (float2*)e[k].d_out_normalized, n, &r.state->gain, &r.state->normalize_coef, st));
+        if (e[k].d_out_no_limiter) MGB_TRY(launch_scale(res, (float2*)e[k].d_out_no_limiter, n, &r.state->gain, nullptr, st));
+    }
+    if (!lim.count) return MGB_OK;
+    MGB_REQUIRE(plan->d_limiter_tables != nullptr, MGB_ERR_INVALID, "versions: the plan has no limiter tables");
+    MGB_TRY(device_zero(ws.tickets, ws.limiter_zero_bytes, st));
+    return launch_limiter_versions(plan->limiter, lim, n, &r.state->gain, &r.state->final_amplitude_coef, &r.state->limiter_engaged,
+                                   ws.tickets, ws.lookback, ws.limiter_planes, plan->d_limiter_tables, r.d, st);
+}
+
+int mgb_finalize_versions_to_loudness(const mgb_plan* plan, const mgb_track_layout* L, const mgb_loudness_params* meter,
+                                      const mgb_loudness_target* target, int32_t entries, const mgb_version_entry* e,
+                                      void* d_workspace, const mgb_track_state* d_state, void* d_versions_ws,
+                                      int64_t versions_ws_bytes, void* d_search_ws, int64_t search_ws_bytes,
+                                      mgb_loudness_target_report* d_report, void* stream) {
+    MGB_TRY(check_plan(plan));
+    MGB_REQUIRE(L != nullptr && d_state != nullptr, MGB_ERR_INVALID, "layout/state is NULL");
+    MGB_TRY(loudness_target_validate(target, meter));
+    MGB_REQUIRE(meter->sample_rate == plan->sample_rate, MGB_ERR_INVALID,
+                "versions to loudness: the meter's rate %d differs from the plan's %d", meter->sample_rate, plan->sample_rate);
+    MGB_REQUIRE(plan->d_limiter_tables != nullptr, MGB_ERR_INVALID, "versions to loudness: the plan has no limiter tables");
+    MGB_TRY(check_version_entries(entries, e, true));
+    MGB_TRY(check_aligned(d_workspace, "d_workspace"));
+    MGB_TRY(check_aligned(d_versions_ws, "d_versions_ws"));
+    MGB_TRY(check_aligned(d_search_ws, "d_search_ws"));
+    MGB_TRY(check_aligned(d_report, "d_report"));
+    const int64_t need = mgb_versions_workspace_bytes(plan, L);
+    MGB_REQUIRE(need > 0, MGB_ERR_INVALID, "versions: the layout has no more than fft_size frames");
+    MGB_REQUIRE(versions_ws_bytes >= need, MGB_ERR_WORKSPACE, "versions: workspace of %lld bytes, need %lld",
+                (long long)versions_ws_bytes, (long long)need);
+    const int64_t n = L->target_frames;
+    const int64_t search_need = loudness_target_search_bytes(*meter, n);
+    MGB_REQUIRE(search_ws_bytes >= search_need, MGB_ERR_WORKSPACE,
+                "versions to loudness: search workspace of %lld bytes, need %lld", (long long)search_ws_bytes,
+                (long long)search_need);
+    cudaStream_t st = (cudaStream_t)stream;
+    const Workspace ws = carve_workspace(*plan, *L, d_workspace);
+    const VersionRegions r = carve_versions(*L, d_versions_ws);
+    VersionPlanes vp;
+    memset(&vp, 0, sizeof(vp));
+    vp.count = entries;
+    for (int k = 0; k < entries; ++k) {
+        vp.in[k] = (const float2*)e[k].d_result_lr;
+        vp.out[k] = (float2*)e[k].d_out_limited;
+    }
+    MGB_TRY(device_zero(ws.tickets, ws.limiter_zero_bytes, st));
+    MGB_TRY(versions_detect(*plan, n, entries, e, r, st));
+    // s = result * gain of the main, metered once from its output (the first pass overwrites it)
+    MGB_TRY(launch_scale(vp.in[0], vp.out[0], n, &d_state->gain, nullptr, st));
+    return run_versions_loudness_search(plan->limiter, *meter, *target, vp, vp.out[0], n, &d_state->gain, r.d_max, r.d, ws.tickets,
+                                        ws.limiter_zero_bytes, ws.lookback, ws.limiter_planes, plan->d_limiter_tables, d_search_ws,
+                                        d_report, st);
+}
+
 int mgb_correct_levels(const mgb_plan* plan, const mgb_track_layout* L, void* d_workspace, mgb_track_state* d_state,
                        void* stream) {
     MGB_TRY(check_plan(plan));

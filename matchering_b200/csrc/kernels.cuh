@@ -177,6 +177,13 @@ int launch_pcm_encode_dithered(const mgb_dither_params& p, const float* in, int6
 int launch_convert_f64_f32(const double* in, float* out, int64_t count, cudaStream_t stream);
 int launch_convert_f32_f64(const float* in, double* out, int64_t count, cudaStream_t stream);
 
+// linked versions (mgb_finalize_versions): the limiter's and the detector's entries, the main first
+struct VersionPlanes {
+    int count;  // 1 + versions
+    const float2* in[1 + MGB_MAX_VERSIONS];
+    float2* out[1 + MGB_MAX_VERSIONS];
+};
+
 // limiter.cu ------------------------------------------------------------------------------------
 // (the halo kernel where its span fits, the wide-window path otherwise; wide_planes: limiter_plane_bytes of workspace)
 int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, int64_t frames, const double* pre_gain,
@@ -193,8 +200,13 @@ int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames);
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
                         void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d,
-                        const int* skip);
+                        const int* skip, const VersionPlanes* vp = nullptr);  // vp: the linked limiter's entries
 int launch_limiter_tables(const mgb_limiter_params& lp, void* tables, cudaStream_t stream);
+// the linked limiter: the gain envelope of the detector plane d (D: max over the entries' detectors), applied to every
+// entry of vp with the same float64 gain; the halo kernel's or the wide-window path's
+int launch_limiter_versions(const mgb_limiter_params& lp, const VersionPlanes& vp, int64_t frames, const double* pre_gain,
+                            const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
+                            const void* tables, const float* d, cudaStream_t stream);
 int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, double threshold, int* engaged,
                            cudaStream_t stream);
 
@@ -202,6 +214,10 @@ int launch_limiter_engaged(const float* peak_bits, const double* pre_gain, doubl
 void true_peak_filter(int oversample, double* h);  // the 12 L + 1 interpolator taps
 int64_t true_peak_plane_bytes(const mgb_limiter_params& lp, int64_t frames);  // the detector plane; 0 without true_peak
 int launch_true_peak_detect(int oversample, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream);
+// d[n] = max(d[n], the detector of x at n) and *d_max = max(*d_max, that): a version's detector added to the main's
+int launch_true_peak_accumulate(int oversample, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream);
+// sample-peak mode's linked detector: d[n] = max over the entries of max(|L|, |R|) at n, and its maximum into *d_max
+int launch_versions_detect(const VersionPlanes& vp, int64_t frames, float* d, float* d_max, cudaStream_t stream);
 int launch_true_peak_final(const float* d_max, double eps, double threshold, mgb_track_state* state, cudaStream_t stream);
 
 // loudness_target.cuh -------------------------------------------------------------------------------
@@ -227,6 +243,12 @@ struct AlbumSearchTrack {
     void* planes;
     const float* tp_d;
 };
+// mgb_finalize_versions_to_loudness: run_loudness_search on entry 0 (the main) with the limiter reading the linked detector
+// plane d (d_max its maximum), then one linked pass at the drive the search ended on, which writes every entry of vp
+int run_versions_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& target,
+                                 const VersionPlanes& vp, const float2* s_metered, int64_t frames, const double* gain,
+                                 const float* d_max, const float* d, void* zero, int64_t zero_bytes, void* lookback, void* planes,
+                                 const void* tables, void* search_ws, mgb_loudness_target_report* report, cudaStream_t stream);
 int64_t album_loudness_target_search_bytes(const mgb_loudness_params& meter, int tracks, const int64_t* frames);
 int run_album_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& target,
                               const AlbumSearchTrack* tracks, int count, const void* tables, void* search_ws,

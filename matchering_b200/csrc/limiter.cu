@@ -135,13 +135,16 @@ __global__ void limiter_tables_kernel(mgb_limiter_params lp, int span_ept, unsig
 // read only where the output is formed.
 // GATED (loudness targets, loudness_target.cuh): the whole grid returns at once while *skip is set -- a pass the
 // search did not need.
-template <int EPT, int NO, bool GAINS = false, bool TP = false, bool GATED = false>
-// (two CTAs per SM where the span leaves room for them: up to 17 samples per thread at order capacity 1)
-__global__ void __launch_bounds__(NT, (NO == 1 && EPT <= 17) ? 2 : 1)
-limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__ in, float2* __restrict__ out,
-               long long frames, const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
-               const int* __restrict__ engaged, int* __restrict__ ticket, LookbackWord* __restrict__ slots,
-               const unsigned char* __restrict__ tables, const float* __restrict__ tp_d, const int* __restrict__ skip) {
+// VERS (linked versions, mgb_finalize_versions): TP's detector plane holds D, the maximum over the main and its versions;
+// every entry of *vp (the main first) takes the same gain in P7 and the same early-out.  limiter_kernel and
+// limiter_versions_kernel below are this body with and without it.
+template <int EPT, int NO, bool GAINS, bool TP, bool GATED, bool VERS>
+__device__ __forceinline__ void
+limiter_body(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__ in, float2* __restrict__ out,
+             long long frames, const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
+             const int* __restrict__ engaged, int* __restrict__ ticket, LookbackWord* __restrict__ slots,
+             const unsigned char* __restrict__ tables, const float* __restrict__ tp_d, const int* __restrict__ skip,
+             const VersionPlanes* vp) {
     if constexpr (GATED) {
         if (*skip) return;
     }
@@ -221,9 +224,17 @@ limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__
         }
     }
     if (bypass) {  // hyrax.py:83-85: the limiter is not needed
-        for (int k = tid; k < core_n; k += NT) {
-            const float2 w = in[s0 + k];
-            out[s0 + k] = make_float2((float)((double)w.x * pre * post), (float)((double)w.y * pre * post));
+        if constexpr (VERS) {
+            for (int j = 0; j < vp->count; ++j)
+                for (int k = tid; k < core_n; k += NT) {
+                    const float2 w = vp->in[j][s0 + k];
+                    vp->out[j][s0 + k] = make_float2((float)((double)w.x * pre * post), (float)((double)w.y * pre * post));
+                }
+        } else {
+            for (int k = tid; k < core_n; k += NT) {
+                const float2 w = in[s0 + k];
+                out[s0 + k] = make_float2((float)((double)w.x * pre * post), (float)((double)w.y * pre * post));
+            }
         }
         return;
     }
@@ -547,7 +558,27 @@ limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__
     // ---- P7: apply (hyrax.py:99, stages.py:203) -----------------------------------------------------
     // The gains sit in shared memory in the filters' mapping (thread t: samples t*CORE_EPT ..); lane l of
     // warp w now takes samples w*32*CORE_EPT + l + 32 q, so that every global access is 32 neighbours.
-    {
+    if constexpr (VERS) {  // the main's gains on every entry, the loads of one entry in flight at a time
+        const int wbase = (tid >> 5) * (32 * CORE_EPT) + (tid & 31);
+        for (int j = 0; j < vp->count; ++j) {
+            const float2* src = vp->in[j];
+            float2* dst = vp->out[j];
+            float2 v[CORE_EPT];
+#pragma unroll
+            for (int q = 0; q < CORE_EPT; ++q) {
+                const int k = wbase + q * 32;
+                v[q] = k < core_n ? __ldg(src + s0 + k) : make_float2(0.0f, 0.0f);
+            }
+#pragma unroll
+            for (int q = 0; q < CORE_EPT; ++q) {
+                const int k = wbase + q * 32;
+                if (k < core_n) {
+                    const double gain = Fd[k] * scale;
+                    dst[s0 + k] = make_float2((float)((double)v[q].x * gain), (float)((double)v[q].y * gain));
+                }
+            }
+        }
+    } else {
         const int wbase = (tid >> 5) * (32 * CORE_EPT) + (tid & 31);
         float2 v[CORE_EPT];
 #pragma unroll
@@ -569,6 +600,28 @@ limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__
             }
         }
     }
+}
+
+template <int EPT, int NO, bool GAINS = false, bool TP = false, bool GATED = false>
+// (two CTAs per SM where the span leaves room for them: up to 17 samples per thread at order capacity 1)
+__global__ void __launch_bounds__(NT, (NO == 1 && EPT <= 17) ? 2 : 1)
+limiter_kernel(mgb_limiter_params lp, LimiterGeom gm, const float2* __restrict__ in, float2* __restrict__ out,
+               long long frames, const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
+               const int* __restrict__ engaged, int* __restrict__ ticket, LookbackWord* __restrict__ slots,
+               const unsigned char* __restrict__ tables, const float* __restrict__ tp_d, const int* __restrict__ skip) {
+    limiter_body<EPT, NO, GAINS, TP, GATED, false>(lp, gm, in, out, frames, pre_gain, post_gain, engaged, ticket, slots, tables,
+                                                   tp_d, skip, nullptr);
+}
+
+// the linked limiter: the detector plane D in, every entry of the table out (the main is entry 0)
+template <int EPT, int NO>
+__global__ void __launch_bounds__(NT, (NO == 1 && EPT <= 17) ? 2 : 1)
+limiter_versions_kernel(mgb_limiter_params lp, LimiterGeom gm, long long frames, const double* __restrict__ pre_gain,
+                        const double* __restrict__ post_gain, const int* __restrict__ engaged, int* __restrict__ ticket,
+                        LookbackWord* __restrict__ slots, const unsigned char* __restrict__ tables,
+                        const float* __restrict__ tp_d, const __grid_constant__ VersionPlanes vp) {
+    limiter_body<EPT, NO, false, true, false, true>(lp, gm, vp.in[0], vp.out[0], frames, pre_gain, post_gain, engaged, ticket,
+                                                    slots, tables, tp_d, nullptr, &vp);
 }
 
 // engaged = not all(isclose(rectified, 1.0)) with numpy's defaults rtol=1e-5, atol=1e-8
@@ -823,6 +876,43 @@ int launch_limiter(const mgb_limiter_params& lp, const float2* in, float2* out, 
     }
 #undef MGB_LIMITER_CASE
     set_error("limiter: no kernel for %d span samples per thread", g.ept);
+    return MGB_ERR_UNSUPPORTED;
+}
+
+int launch_limiter_versions(const mgb_limiter_params& lp, const VersionPlanes& vp, int64_t frames, const double* pre_gain,
+                            const double* post_gain, const int* engaged, int* ticket, void* lookback, void* wide_planes,
+                            const void* tables, const float* d, cudaStream_t stream) {
+    MGB_TRY(limiter_validate(lp));
+    MGB_REQUIRE(frames > 6, MGB_ERR_INVALID, "limiter: the input must be longer than filtfilt's padlen (6)");
+    MGB_REQUIRE(tables != nullptr && d != nullptr, MGB_ERR_INVALID, "limiter (versions): pole tables or detector plane missing");
+    MGB_REQUIRE(vp.count >= 1 && vp.count <= 1 + MGB_MAX_VERSIONS, MGB_ERR_INVALID, "limiter (versions): %d entries", vp.count);
+    if (limiter_span_too_wide(lp))
+        return launch_limiter_wide(lp, limiter_order_capacity(lp), g_lookback_inclusive, vp.in[0], vp.out[0], frames, pre_gain,
+                                   post_gain, engaged, lookback, wide_planes, tables, stream, false, d, nullptr, &vp);
+    LimiterGeom g;
+    MGB_TRY(limiter_geometry(lp, &g));
+    const int64_t chunks = (frames + LC - 1) / LC;
+    const size_t smem = (size_t)g.ept * NT * 16 + (size_t)g.margin * 8;
+    const int no = limiter_order_capacity(lp);
+    auto run = [&](auto kernel) {
+        return launch("limiter_versions_kernel", kernel, dim3((unsigned)chunks), dim3(NT), smem, stream, lp, g, (long long)frames,
+                      pre_gain, post_gain, engaged, ticket, (LookbackWord*)lookback, (const unsigned char*)tables, d, vp);
+    };
+#define MGB_LIMITER_CASE(E) \
+    case E: return no == 1 ? run(limiter_versions_kernel<E, 1>) : run(limiter_versions_kernel<E, MGB_MAX_FILTER_ORDER>);
+    switch (g.ept) {
+        MGB_LIMITER_CASE(11)
+        MGB_LIMITER_CASE(13)
+        MGB_LIMITER_CASE(15)
+        MGB_LIMITER_CASE(17)
+        MGB_LIMITER_CASE(19)
+        MGB_LIMITER_CASE(21)
+        MGB_LIMITER_CASE(23)
+        MGB_LIMITER_CASE(25)
+        default: break;
+    }
+#undef MGB_LIMITER_CASE
+    set_error("limiter (versions): no kernel for %d span samples per thread", g.ept);
     return MGB_ERR_UNSUPPORTED;
 }
 

@@ -223,12 +223,14 @@ __global__ void __launch_bounds__(NT) limiter_wide_attack_kernel(mgb_limiter_par
 
 // Hold and release sections (limiter.cu, P3 / P5 / P6: the same scans and look-back) over H from the window
 // maxima, then the gain and its application (P7).  GAINS (tests): write (g_att, max(hold_out, release_out)).
-template <int NO, bool GAINS, bool GATED = false>
-__global__ void __launch_bounds__(NT) limiter_wide_apply_kernel(mgb_limiter_params lp, WideGeom w, const float2* __restrict__ in,
-                                                                float2* __restrict__ out, const double* __restrict__ pre_gain,
-                                                                const double* __restrict__ post_gain, const int* __restrict__ engaged,
-                                                                WidePlanes p, LookbackWord* __restrict__ slots,
-                                                                const unsigned char* __restrict__ tables, const int* __restrict__ skip) {
+// VERS (linked versions): every entry of *vp (the main first) takes the same gain and the same early-out.
+template <int NO, bool GAINS, bool GATED, bool VERS>
+__device__ __forceinline__ void limiter_wide_apply_body(mgb_limiter_params lp, WideGeom w,
+                                                        const float2* __restrict__ in, float2* __restrict__ out,
+                                                        const double* __restrict__ pre_gain, const double* __restrict__ post_gain,
+                                                        const int* __restrict__ engaged, WidePlanes p,
+                                                        LookbackWord* __restrict__ slots, const unsigned char* __restrict__ tables,
+                                                        const int* __restrict__ skip, const VersionPlanes* vp) {
     if (skipped<GATED>(skip)) return;
     constexpr int HC = CORE_EPT + NO;
     __shared__ SectionTab<1> pw_sec[2];  // (order capacity 1 only: the two sections' tables)
@@ -245,9 +247,17 @@ __global__ void __launch_bounds__(NT) limiter_wide_apply_kernel(mgb_limiter_para
     const double pre = pre_gain ? *pre_gain : 1.0;
     const double post = post_gain ? *post_gain : 1.0;
     if (bypassed(engaged)) {  // hyrax.py:83-85: the limiter is not needed
-        for (int k = tid; k < core_n; k += NT) {
-            const float2 v = in[s0 + k];
-            out[s0 + k] = make_float2((float)((double)v.x * pre * post), (float)((double)v.y * pre * post));
+        if constexpr (VERS) {
+            for (int j = 0; j < vp->count; ++j)
+                for (int k = tid; k < core_n; k += NT) {
+                    const float2 v = vp->in[j][s0 + k];
+                    vp->out[j][s0 + k] = make_float2((float)((double)v.x * pre * post), (float)((double)v.y * pre * post));
+                }
+        } else {
+            for (int k = tid; k < core_n; k += NT) {
+                const float2 v = in[s0 + k];
+                out[s0 + k] = make_float2((float)((double)v.x * pre * post), (float)((double)v.y * pre * post));
+            }
         }
         return;
     }
@@ -381,15 +391,53 @@ __global__ void __launch_bounds__(NT) limiter_wide_apply_kernel(mgb_limiter_para
     // ---- apply (hyrax.py:99, stages.py:203), coalesced as in the halo kernel
     const double scale = pre * post;
     const int wbase = (tid >> 5) * (32 * CORE_EPT) + (tid & 31);
+    if constexpr (VERS) {
+        for (int j = 0; j < vp->count; ++j) {
+            const float2* src = vp->in[j];
+            float2* dst = vp->out[j];
 #pragma unroll
-    for (int q = 0; q < CORE_EPT; ++q) {
-        const int k = wbase + q * 32;
-        if (k < core_n) {
-            const float2 v = __ldg(in + s0 + k);
-            const double gain = gain_s[k] * scale;
-            out[s0 + k] = make_float2((float)((double)v.x * gain), (float)((double)v.y * gain));
+            for (int q = 0; q < CORE_EPT; ++q) {
+                const int k = wbase + q * 32;
+                if (k < core_n) {
+                    const float2 v = __ldg(src + s0 + k);
+                    const double gain = gain_s[k] * scale;
+                    dst[s0 + k] = make_float2((float)((double)v.x * gain), (float)((double)v.y * gain));
+                }
+            }
+        }
+    } else {
+#pragma unroll
+        for (int q = 0; q < CORE_EPT; ++q) {
+            const int k = wbase + q * 32;
+            if (k < core_n) {
+                const float2 v = __ldg(in + s0 + k);
+                const double gain = gain_s[k] * scale;
+                out[s0 + k] = make_float2((float)((double)v.x * gain), (float)((double)v.y * gain));
+            }
         }
     }
+}
+
+template <int NO, bool GAINS, bool GATED = false>
+__global__ void __launch_bounds__(NT) limiter_wide_apply_kernel(mgb_limiter_params lp, WideGeom w, const float2* __restrict__ in,
+                                                                float2* __restrict__ out, const double* __restrict__ pre_gain,
+                                                                const double* __restrict__ post_gain, const int* __restrict__ engaged,
+                                                                WidePlanes p, LookbackWord* __restrict__ slots,
+                                                                const unsigned char* __restrict__ tables, const int* __restrict__ skip) {
+    limiter_wide_apply_body<NO, GAINS, GATED, false>(lp, w, in, out, pre_gain, post_gain, engaged, p, slots, tables, skip, nullptr);
+}
+
+// the linked limiter's apply step (limiter_versions_kernel's P7 and early-out on the wide-window path)
+template <int NO>
+__global__ void __launch_bounds__(NT) limiter_wide_apply_versions_kernel(mgb_limiter_params lp, WideGeom w,
+                                                                         const double* __restrict__ pre_gain,
+                                                                         const double* __restrict__ post_gain,
+                                                                         const int* __restrict__ engaged, WidePlanes p,
+                                                                         LookbackWord* __restrict__ slots,
+                                                                         const unsigned char* __restrict__ tables,
+                                                                         const __grid_constant__ VersionPlanes vp) {
+    limiter_wide_apply_body<NO, false, false, true>(lp, w, vp.in[0], vp.out[0], pre_gain, post_gain, engaged, p, slots, tables,
+                                                    nullptr, &vp);
 }
 
 struct WideLayout {
@@ -439,7 +487,7 @@ int64_t limiter_wide_plane_bytes(const mgb_limiter_params& lp, int64_t frames) {
 int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int publish_inclusive, const float2* in, float2* out,
                         int64_t frames, const double* pre_gain, const double* post_gain, const int* engaged, void* lookback,
                         void* planes, const void* tables, cudaStream_t stream, bool gains_only, const float* tp_d,
-                        const int* skip) {
+                        const int* skip, const VersionPlanes* vp) {
     MGB_REQUIRE(planes != nullptr, MGB_ERR_INVALID, "limiter (wide windows): workspace planes missing");
     const WideLayout L = wide_layout(lp, frames);
     unsigned char* base = (unsigned char*)planes;
@@ -480,6 +528,14 @@ int launch_limiter_wide(const mgb_limiter_params& lp, int order_capacity, int pu
     };
     MGB_TRY(skip ? attack(limiter_wide_attack_kernel<false, true>) : attack(limiter_wide_attack_kernel<false>));
     MGB_TRY(skip ? attack(limiter_wide_attack_kernel<true, true>) : attack(limiter_wide_attack_kernel<true>));
+    if (vp) {
+        auto linked = [&](auto kernel) {
+            return launch("limiter_wide_apply_versions_kernel", kernel, dim3((unsigned)L.chunks), dim3(NT), 0, stream, lp, w,
+                          pre_gain, post_gain, engaged, p, sec_words, tab, *vp);
+        };
+        return order_capacity == 1 ? linked(limiter_wide_apply_versions_kernel<1>)
+                                   : linked(limiter_wide_apply_versions_kernel<MGB_MAX_FILTER_ORDER>);
+    }
     auto go = [&](auto kernel) {
         return launch("limiter_wide_apply_kernel", kernel, dim3((unsigned)L.chunks), dim3(NT), 0, stream, lp, w, in, out, pre_gain,
                       post_gain, engaged, p, sec_words, tab, skip);

@@ -251,6 +251,29 @@ int run_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params&
     return MGB_OK;
 }
 
+// Linked versions (mgb_finalize_versions_to_loudness): the main's search, unchanged, with its limiter reading the linked
+// detector plane d (set true_peak so the kernels that take the plane serve it; in sample-peak mode d holds max(|L|, |R|),
+// which P1 rectifies exactly as the sample path does) and its early-out taking max(d).  The header then holds the drive
+// and the early-out flag of the pass the search ended on: one linked pass there writes every entry, the main's samples
+// being that pass's own.
+int run_versions_loudness_search(const mgb_limiter_params& lp, const mgb_loudness_params& meter, const mgb_loudness_target& t,
+                                 const VersionPlanes& vp, const float2* s_metered, int64_t frames, const double* gain,
+                                 const float* d_max, const float* d, void* zero, int64_t zero_bytes, void* lookback, void* planes,
+                                 const void* tables, void* search_ws, mgb_loudness_target_report* report, cudaStream_t st) {
+    mgb_limiter_params lpd = lp;
+    if (!lpd.true_peak) lpd.true_peak = 1;
+    MGB_TRY(run_loudness_search(lpd, meter, t, vp.in[0], s_metered, vp.out[0], frames, gain, nullptr, d_max, zero, zero_bytes,
+                                nullptr, lookback, planes, tables, d, search_ws, report, st));
+    TargetSearch* s = (TargetSearch*)search_ws;
+#ifdef MGB_EMULATE
+    memset(zero, 0, zero_bytes);
+#else
+    if (cudaMemsetAsync(zero, 0, zero_bytes, st) != cudaSuccess) return cuda_status("memset");
+#endif
+    return launch_limiter_versions(lp, vp, frames, &s->pre_gain, nullptr, &s->engaged, (int*)zero, lookback, planes, tables, d,
+                                   st);
+}
+
 int64_t album_loudness_target_search_bytes(const mgb_loudness_params& meter, int tracks, const int64_t* frames) {
     MeterWorkspace w[MGB_MAX_ALBUM_TRACKS];
     return kAlbumTargetHeader + carve_album_meter(meter, tracks, frames, nullptr, w).total;

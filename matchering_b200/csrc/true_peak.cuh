@@ -76,6 +76,75 @@ __global__ void __launch_bounds__(kTpThreads) true_peak_detect_kernel(TruePeakTa
     if (tid == 0) atomic_max_nonneg(d_max, pk);
 }
 
+// true_peak_detect_kernel for a version of the main (linked versions): d[n] = max(d[n], its detector at n).  A copy of
+// that kernel rather than a flag on it, which changed its register allocation.
+template <int OS>
+__global__ void __launch_bounds__(kTpThreads) true_peak_accumulate_kernel(TruePeakTaps taps, const float2* __restrict__ x,
+                                                                          long long frames, float* __restrict__ d,
+                                                                          float* __restrict__ d_max) {
+    __shared__ float2 xs[kTpTile + 2 * kTpHalo];  // frames s0 - 6 .. s0 + kTpTile + 5, zero outside the signal
+    __shared__ float us[kTpTile + 1];             // u at frames s0 - 1 .. s0 + kTpTile - 1
+    __shared__ float red[32];
+    const int tid = threadIdx.x;
+    const long long s0 = (long long)blockIdx.x * kTpTile;
+    for (int i = tid; i < kTpTile + 2 * kTpHalo; i += kTpThreads) {
+        const long long n = s0 - kTpHalo + i;
+        xs[i] = (n >= 0 && n < frames) ? __ldg(x + n) : make_float2(0.0f, 0.0f);
+    }
+    __syncthreads();
+    for (int i = tid; i <= kTpTile; i += kTpThreads) {
+        const long long n = s0 - 1 + i;  // frame n sits at xs[i + 5]
+        float m = 0.0f;
+        if (n >= 0 && n < frames) {
+            const float2 c = xs[i + 5];
+            m = fmaxf(fabsf(c.x), fabsf(c.y));
+#pragma unroll
+            for (int ph = 1; ph < OS; ++ph) {
+                float aL = 0.0f, aR = 0.0f;
+#pragma unroll
+                for (int t = -5; t <= 6; ++t) {
+                    const float2 v = xs[i + 5 + t];
+                    aL = fmaf(taps.w[ph - 1][t + 5], v.x, aL);
+                    aR = fmaf(taps.w[ph - 1][t + 5], v.y, aR);
+                }
+                m = fmaxf(m, fmaxf(fabsf(aL), fabsf(aR)));
+            }
+        }
+        us[i] = m;
+    }
+    __syncthreads();
+    float pk = 0.0f;
+    for (int j = tid; j < kTpTile; j += kTpThreads) {
+        const long long n = s0 + j;
+        if (n < frames) {
+            const float v = fmaxf(d[n], fmaxf(us[j + 1], us[j]));
+            d[n] = v;
+            pk = fmaxf(pk, v);
+        }
+    }
+    pk = block_max(pk, red);
+    if (tid == 0) atomic_max_nonneg(d_max, pk);
+}
+
+// sample-peak mode's linked detector: d[n] = max over the entries of max(|L|, |R|), one read of every entry per frame
+__global__ void __launch_bounds__(256) versions_detect_kernel(const __grid_constant__ VersionPlanes vp, long long frames,
+                                                              float* __restrict__ d, float* __restrict__ d_max) {
+    __shared__ float red[32];
+    float pk = 0.0f;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < frames; n += stride) {
+        float m = 0.0f;
+        for (int j = 0; j < vp.count; ++j) {
+            const float2 v = __ldg(vp.in[j] + n);
+            m = fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y)));
+        }
+        d[n] = m;
+        pk = fmaxf(pk, m);
+    }
+    pk = block_max(pk, red);
+    if (threadIdx.x == 0) atomic_max_nonneg(d_max, pk);
+}
+
 // correction_final_kernel's normalisation coefficient and early-out flag (correct.cu), from the true peak instead of
 // the sample peak: peak = gain * max(d)
 __global__ void true_peak_final_kernel(const float* __restrict__ d_max, double eps, double threshold,
@@ -116,14 +185,19 @@ int64_t true_peak_plane_bytes(const mgb_limiter_params& lp, int64_t frames) {
     return lp.true_peak ? (frames * 4 + 255) / 256 * 256 : 0;
 }
 
-// d_max must hold 0 (or a smaller true peak) before the launch
-int launch_true_peak_detect(int os, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream) {
+static TruePeakTaps true_peak_taps(int os) {
     double h[49];
     true_peak_filter(os, h);
     TruePeakTaps taps;
     memset(&taps, 0, sizeof(taps));
     for (int ph = 1; ph < os; ++ph)
         for (int t = -5; t <= 6; ++t) taps.w[ph - 1][t + 5] = (float)h[(6 - t) * os + ph];
+    return taps;
+}
+
+// d_max must hold 0 (or a smaller true peak) before the launch
+int launch_true_peak_detect(int os, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream) {
+    const TruePeakTaps taps = true_peak_taps(os);
     const dim3 grid((unsigned)((frames + kTpTile - 1) / kTpTile));
     if (os == 4)
         return launch("true_peak_detect_kernel", true_peak_detect_kernel<4>, grid, dim3(kTpThreads), 0, stream, taps, x,
@@ -133,6 +207,27 @@ int launch_true_peak_detect(int os, const float2* x, int64_t frames, float* d, f
                       (long long)frames, d, d_max);
     return launch("true_peak_detect_kernel", true_peak_detect_kernel<1>, grid, dim3(kTpThreads), 0, stream, taps, x,
                   (long long)frames, d, d_max);
+}
+
+int launch_true_peak_accumulate(int os, const float2* x, int64_t frames, float* d, float* d_max, cudaStream_t stream) {
+    const TruePeakTaps taps = true_peak_taps(os);
+    const dim3 grid((unsigned)((frames + kTpTile - 1) / kTpTile));
+    if (os == 4)
+        return launch("true_peak_accumulate_kernel", true_peak_accumulate_kernel<4>, grid, dim3(kTpThreads), 0, stream, taps, x,
+                      (long long)frames, d, d_max);
+    if (os == 2)
+        return launch("true_peak_accumulate_kernel", true_peak_accumulate_kernel<2>, grid, dim3(kTpThreads), 0, stream, taps, x,
+                      (long long)frames, d, d_max);
+    return launch("true_peak_accumulate_kernel", true_peak_accumulate_kernel<1>, grid, dim3(kTpThreads), 0, stream, taps, x,
+                  (long long)frames, d, d_max);
+}
+
+// d_max must hold 0 before the launch
+int launch_versions_detect(const VersionPlanes& vp, int64_t frames, float* d, float* d_max, cudaStream_t stream) {
+    const long long blocks = (frames + 1023) / 1024;  // four frames per thread
+    const unsigned grid = (unsigned)(blocks < 4LL * num_sms() ? (blocks > 0 ? blocks : 1) : 4LL * num_sms());
+    return launch("versions_detect_kernel", versions_detect_kernel, dim3(grid), dim3(256), 0, stream, vp, (long long)frames, d,
+                  d_max);
 }
 
 int launch_true_peak_final(const float* d_max, double eps, double threshold, mgb_track_state* state, cudaStream_t stream) {

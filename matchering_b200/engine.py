@@ -294,6 +294,60 @@ def album_finalize_to_loudness(sessions: list, target_lufs: float, need_no_limit
     return [(lim, plain, normalized) for lim, (_, plain, normalized) in zip(limited, outs)], report
 
 
+def versions_match(main: TrackSession, sessions: list, targets: list) -> None:
+    """Stage 2 of each version with the main's FIR (mgb_version_match_frequencies), after the main's correct_levels: one
+    profiled TrackSession per version, of the main's frame count, and its target on the device."""
+    n = len(sessions)
+    table = (_native.VersionTrack * n)()
+    for entry, session, target in zip(table, sessions, targets):
+        entry.layout = C.pointer(session.layout)
+        entry.d_target_lr, entry.d_result_lr = target.data_ptr(), session.result.data_ptr()
+        entry.d_workspace, entry.d_state = session.workspace.data_ptr(), session.state.data_ptr()
+    p, l = main._args()
+    _native.check(main.lib, main.lib.mgb_version_match_frequencies(p, l, main.workspace.data_ptr(), main.state.data_ptr(), n,
+                                                                    table, _stream_ptr(main.device)))
+
+
+def versions_finalize(main: TrackSession, results: list, need_default: bool, need_no_limiter: bool,
+                      need_no_limiter_normalized: bool, loudness_target: float | None = None):
+    """Stage 4 of the main (results[0], its own result) and its versions with one detector and one gain envelope
+    (mgb_finalize_versions; with loudness_target the limited outputs at the main's searched drive,
+    mgb_finalize_versions_to_loudness).  -> ([(limited, plain, normalized) per entry], the device report or None)"""
+    lib, dev = main.lib, main.device
+    n, count = main.layout.target_frames, len(results)
+    p, l = main._args()
+    vbytes = int(lib.mgb_versions_workspace_bytes(p, l))
+    if vbytes < 0:
+        raise ValueError(lib.mgb_last_error_string().decode("utf-8", "replace"))
+    vws = torch.empty(vbytes, dtype=torch.uint8, device=dev)
+    mk = lambda need: torch.empty((n, 2), dtype=torch.float32, device=dev) if need else None
+    targeted = need_default and loudness_target is not None
+    outs = [(mk(need_default), mk(need_no_limiter), mk(need_no_limiter_normalized)) for _ in results]
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    table = (_native.VersionEntry * count)()
+    for entry, result, (lim, plain, norm) in zip(table, results, outs):
+        entry.d_result_lr = result.data_ptr()
+        entry.d_out_limited = None if targeted else ptr(lim)
+        entry.d_out_no_limiter, entry.d_out_normalized = ptr(plain), ptr(norm)
+    report = None
+    if any(t is not None for entry in outs for t in entry) and (not targeted or need_no_limiter or need_no_limiter_normalized):
+        _native.check(lib, lib.mgb_finalize_versions(p, l, count, table, main.workspace.data_ptr(), main.state.data_ptr(),
+                                                     vws.data_ptr(), vbytes, _stream_ptr(dev)))
+    if targeted:
+        from .loudness import device_meter, target_params
+        for entry, (lim, _, _) in zip(table, outs):
+            entry.d_out_limited, entry.d_out_no_limiter, entry.d_out_normalized = lim.data_ptr(), None, None
+        meter = device_meter(main.plan.tables.sample_rate, dev)
+        search_bytes = int(lib.mgb_loudness_target_workspace_bytes(C.byref(meter.params), n))
+        search = torch.empty(search_bytes, dtype=torch.uint8, device=dev)
+        report = torch.empty(C.sizeof(_native.LoudnessTargetReport), dtype=torch.uint8, device=dev)
+        _native.check(lib, lib.mgb_finalize_versions_to_loudness(
+            p, l, C.byref(meter.params), C.byref(target_params(loudness_target)), count, table, main.workspace.data_ptr(),
+            main.state.data_ptr(), vws.data_ptr(), vbytes, search.data_ptr(), search_bytes, report.data_ptr(),
+            _stream_ptr(dev)))
+    return outs, report
+
+
 # ------------------------------------------------------------------------------------------------
 # host arrays in, host arrays out (the reference's seam: pageable float64 numpy, core.py:77-86)
 # ------------------------------------------------------------------------------------------------

@@ -10,7 +10,7 @@ import torch
 from . import _native, plan as _plan
 from .defaults import Config
 from .engine import (TrackSession, album_finalize_to_loudness, album_match, get_native_plan, get_plan, host_array_ok, stages_main_host,
-                     stages_main_host_profiled, to_device_f32, to_host_like)
+                     stages_main_host_profiled, to_device_f32, to_host_like, versions_finalize, versions_match)
 from .log import Code, info, debug, debug_line, debug_enabled
 from .profile import ReferenceProfile
 from .utils import to_db
@@ -302,3 +302,89 @@ def main_album_device(targets, reference, config: Config, need_default: bool = T
                 debug_target(LoudnessTarget.from_report(float(album_loudness_target),
                                                         _native.LoudnessTargetReport.from_buffer_copy(raw)))
     return outs
+
+
+def main_versions(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
+                  need_no_limiter_normalized: bool = False):
+    """Master a mix (targets[0]) and its versions -- instrumental, a cappella, TV mix, clean edit -- as linked versions
+    (DESIGN.md section 4 "Linked versions"): the level and spectrum match is the main's alone, every version goes through
+    the main's FIR and correction gain, and one limiter gain envelope, computed from the loudest of all their detectors
+    at every frame, limits every one of them.  So main - instrumental is the vocal through the same chain.  targets:
+    (N, 2) stereo arrays of ONE frame count at config.internal_sample_rate, numpy or torch; reference: samples or a
+    ReferenceProfile.  Returns one (result, result_no_limiter, result_no_limiter_normalized) per target, None where not
+    requested, in each target's array type.  Where no version is louder than the main at any frame, the main's outputs
+    are `main`'s bit for bit.  Config(loudness_target=T) searches the main's limited output to T and gives every
+    version the same drive."""
+    outs = main_versions_device(targets, reference, config, need_default, need_no_limiter, need_no_limiter_normalized)
+    return [tuple(None if t is None else to_host_like(t, target) for t in entry) for entry, target in zip(outs, targets)]
+
+
+def versions_check(targets, config: Config) -> None:
+    """The version requests main_versions refuses before any device work."""
+    if len(targets) < 1:
+        raise ValueError("linked versions need the main mix")
+    if len(targets) - 1 > _native.MGB_MAX_VERSIONS:
+        raise ValueError(f"{len(targets) - 1} versions: at most {_native.MGB_MAX_VERSIONS} are linked to one main mix")
+    for target in targets:
+        if target.ndim != 2 or target.shape[1] != 2:
+            raise ValueError("every target must be a (frames, 2) stereo array")
+    n = int(targets[0].shape[0])
+    if not n > config.fft_size:
+        raise ValueError(f"the main mix must be longer than fft_size ({config.fft_size} frames)")
+    for k, target in enumerate(targets[1:], 1):
+        if int(target.shape[0]) != n:
+            raise ValueError(f"version {k} has {int(target.shape[0])} frames, the main mix {n}: linked versions share "
+                             "the main's frame count")
+
+
+def main_versions_device(targets, reference, config: Config, need_default: bool = True, need_no_limiter: bool = False,
+                         need_no_limiter_normalized: bool = False):
+    """`main_versions` with the results left on the device as float32 CUDA tensors."""
+    targets = list(targets)
+    versions_check(targets, config)
+    profiled = isinstance(reference, ReferenceProfile)
+    if profiled:
+        reference.check_config(config)
+    elif reference.ndim != 2 or reference.shape[1] != 2:
+        raise ValueError("the reference must be a (frames, 2) stereo array")
+    plan = get_plan(config)
+    device = plan.device
+    with torch.cuda.device(device):
+        d_targets = [to_device_f32(t, device) for t in targets]
+        n = int(d_targets[0].shape[0])
+        if profiled:
+            d_profile = reference.checked_blob(plan)
+            main = TrackSession(plan, n, None)
+        else:
+            d_reference = to_device_f32(reference, device)
+            main = TrackSession(plan, n, int(d_reference.shape[0]))
+        versions = [TrackSession(plan, n, None) for _ in d_targets[1:]]
+
+        debug_line()
+        info(Code.INFO_MATCHING_LEVELS)
+        debug(f"The main mix and {len(versions)} linked versions of {n} frames")
+        if profiled:
+            main.match_levels_profiled(d_targets[0], d_profile)
+        else:
+            main.match_levels(d_targets[0], d_reference)
+        debug_line()
+        info(Code.INFO_MATCHING_FREQS)
+        main.match_frequencies(d_targets[0])
+        debug_line()
+        info(Code.INFO_CORRECTING_LEVELS)
+        main.correct_levels()
+        if versions:
+            versions_match(main, versions, d_targets[1:])
+
+        debug_line()
+        info(Code.INFO_FINALIZING)
+        outs, report = versions_finalize(main, [main.result] + [v.result for v in versions], need_default, need_no_limiter,
+                                         need_no_limiter_normalized, config.loudness_target)
+        if debug_enabled():
+            _debug_scalars(main.read_state(), main.layout, reference if profiled else None)
+            if report is not None:
+                from .loudness import LoudnessTarget, debug_target
+                raw = report.cpu().numpy().tobytes()
+                debug_target(LoudnessTarget.from_report(config.loudness_target,
+                                                        _native.LoudnessTargetReport.from_buffer_copy(raw)))
+    return [tuple(entry) for entry in outs]
